@@ -209,6 +209,8 @@ int b200sqp_set_builder(b200sqp_handle h, const b200sqp_builder_desc* desc);
  *   handle is the previous primal solution and is shifted by the reference's rule (Initialization.cpp:35-79) -- no host copy of x / u.
  *   With warm = 1, x0 may be NULL: the measured state is then the previous plan interpolated at t0 on the device (perfect tracking, the dummy
  *   simulation of the reference's launch files), which closes the MPC loop without any per-cycle state transfer.
+ *   warm = 2: warm start as with warm = 1, the measured state being the simulated state of the last b200sqp_rollout_policy of this batch (x0 must
+ *   be NULL; B200SQP_ESTATE without such a roll-out): the closed loop of the reference's dummy simulation (MPC, roll-out, MPC, ...) on the device.
  * Every instance must produce the same number of shooting nodes (same event count inside the horizon); *n_nodes returns it, B200SQP_EINVAL
  * otherwise (group such instances by gait phase on the host).  Host pointers; ~0.5 kB per instance cross PCIe. */
 int b200sqp_build_instances(b200sqp_handle h, int batch, double t0, double horizon, const double* x0, const int32_t* gait, const double* gait_start,
@@ -219,6 +221,35 @@ int b200sqp_build_instances(b200sqp_handle h, int batch, double t0, double horiz
  * Any pointer may be NULL. */
 int b200sqp_download_instances(b200sqp_handle h, double* x0, double* x_init, double* u_init, double* t_nodes, uint8_t* node_event, uint8_t* contact_flags,
                                double* swing_ref, double* impact_factor, double* arm_phase, double* x_ref);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Policy roll-out (SURVEY.md section 8(f)-2): MRT_BASE::rolloutPolicy (ocs2_mpc/src/MRT_BASE.cpp:124-151) of the reference's dummy
+ * simulation, batched: TimeTriggeredRollout (ocs2_oc/src/rollout/TimeTriggeredRollout.cpp:46-116) with the OCP's whole-body flow map under the
+ * policy of the last solve -- the LinearController u = bias(t) + K(t) x when settings.use_feedback_policy = 1, the FeedforwardController
+ * otherwise -- integrated by the Dormand-Prince 5(4) stepper of ocs2 (ODE45_OCS2, ocs2_core/src/integration/RungeKuttaDormandPrince5.cpp).
+ * The event times are the plan's PreEvent node times; the jump map is the identity.
+ * ------------------------------------------------------------------------------------------------------------------ */
+/* rollout::Settings fields of the ODE45 roll-out (ocs2_oc/include/ocs2_oc/rollout/RolloutSettings.h) */
+typedef struct b200sqp_rollout_settings {
+  double abs_tol, rel_tol;        /* AbsTolODE, RelTolODE */
+  double time_step;               /* timeStep: initial step of every integration interval */
+  double max_steps_per_second;    /* maxNumStepsPerSecond: flow-map call budget = this * max(1, duration) */
+} b200sqp_rollout_settings;
+/* the G1 whole-body task.info values: 1e-5, 1e-3, 0.015, 10000 */
+void b200sqp_default_rollout_settings(b200sqp_rollout_settings* rs);
+
+/* Simulates every instance from time t for `duration` seconds under the policy of the handle's last solve, ASYNCHRONOUS on `stream` like
+ * b200sqp_solve (b200sqp_wait collects it; so does every entry point that waits for the handle).
+ *   x_start [B][nx] host, or NULL for the handle's current measured state x0;
+ *   outputs (host, each may be NULL, valid after b200sqp_wait): x_end [B][nx], u_end [B][nu] (the policy's input at the last sample),
+ *   mode_end [B] (ModeSchedule::modeAtTime(t + duration): 0 FLY, 1 RF, 2 LF, 3 STANCE), n_steps [B][3] (accepted steps, rejected steps,
+ *   flow-map calls), status [B] (0 ok; 1 more than 100 retries of one step; 2 the flow-map call budget was exceeded; 3 a non-finite state or
+ *   input; the reference throws in these cases, here x_end holds the last accepted state).
+ * The simulated state stays on the device as the handle's simulated measured state, which b200sqp_build_instances(warm = 2) takes as x0.
+ * Like the reference, a t + duration past the plan's last node is not an error: the policy is held at its last node.
+ * Needs a finished b200sqp_solve (B200SQP_ESTATE otherwise); whole-body handles only (B200SQP_EINVAL on a centroidal handle). */
+int b200sqp_rollout_policy(b200sqp_handle h, double t, double duration, const double* x_start, const b200sqp_rollout_settings* rs, double* x_end,
+                           double* u_end, int32_t* mode_end, int32_t* n_steps, int32_t* status, void* stream);
 
 /* per-instance iteration record: mirrors sqp::LogEntry / PerformanceIndex (SqpLogging.h, PerformanceIndex.h) */
 typedef struct b200sqp_iter_log {

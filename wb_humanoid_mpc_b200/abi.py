@@ -92,6 +92,24 @@ class IterLog(C.Structure):
                                           "step_size", "step_type", "dx_norm", "du_norm", "armijo", "convergence")] + [("pad", C.c_double * 2)]
 
 
+class RolloutSettings(C.Structure):
+    _fields_ = [
+        ("abs_tol", C.c_double),
+        ("rel_tol", C.c_double),
+        ("time_step", C.c_double),
+        ("max_steps_per_second", C.c_double),
+    ]
+
+
+def default_rollout_settings(**over) -> RolloutSettings:
+    """rollout::Settings of the G1 whole-body task.info (ODE45, AbsTolODE 1e-5, RelTolODE 1e-3, timeStep 0.015, maxNumStepsPerSecond 10000),
+    then keyword overrides."""
+    s = RolloutSettings(abs_tol=1e-5, rel_tol=1e-3, time_step=0.015, max_steps_per_second=10000.0)
+    for k, v in over.items():
+        setattr(s, k, v)
+    return s
+
+
 def default_settings(model: dict | None = None, **over) -> Settings:
     """sqp::Settings defaults (SqpSettings.h:42-86) overridden by the G1 task.info values, then by keyword arguments."""
     s = Settings(sqp_iteration=1, delta_tol=1e-4, cost_tol=1e-4, alpha_decay=0.5, alpha_min=1e-4, gamma_c=1e-6, g_max=1e-2, g_min=1e-6,

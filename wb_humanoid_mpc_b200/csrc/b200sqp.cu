@@ -19,6 +19,7 @@
 #ifdef B200SQP_WITH_WB
 #include "wb_solver.cuh"
 #include "wb_builder.cuh"
+#include "wb_sim.cuh"
 #include "cen_dynamics.cuh"
 #include "wb_torque.cuh"
 #include "cen_kernels.cuh"
@@ -296,6 +297,15 @@ void b200sqp_default_settings(b200sqp_settings* s) {
   s->use_feedback_policy = 0;
   s->global_step = 0;
   s->create_value_function = 0;
+}
+
+void b200sqp_default_rollout_settings(b200sqp_rollout_settings* rs) {
+  if (!rs) return;
+  // the rollout block of the G1 whole-body task.info (robot_models/unitree_g1/g1_wb_mpc/config/mpc/task.info:97-105)
+  rs->abs_tol = 1e-5;
+  rs->rel_tol = 1e-3;
+  rs->time_step = 0.015;
+  rs->max_steps_per_second = 10000;
 }
 
 }  // extern "C"

@@ -87,14 +87,14 @@ def lib() -> C.CDLL:
         except AttributeError:  # reported by tests/test_abi.py; do not mask the symbols that do exist
             continue
         if name not in ("b200sqp_last_error", "b200sqp_version", "b200sqp_qp_destroy", "b200sqp_destroy", "b200sqp_default_settings",
-                        "b200sqp_host_alloc", "b200sqp_host_free"):
+                        "b200sqp_default_rollout_settings", "b200sqp_host_alloc", "b200sqp_host_free"):
             fn.restype = C.c_int
     if hasattr(L, "b200sqp_host_alloc"):
         L.b200sqp_host_alloc.restype = C.c_void_p
         L.b200sqp_host_alloc.argtypes = [C.c_size_t]
         L.b200sqp_host_free.restype = None
         L.b200sqp_host_free.argtypes = [C.c_void_p]
-    for name in ("b200sqp_qp_destroy", "b200sqp_destroy", "b200sqp_default_settings"):
+    for name in ("b200sqp_qp_destroy", "b200sqp_destroy", "b200sqp_default_settings", "b200sqp_default_rollout_settings"):
         if hasattr(L, name):
             getattr(L, name).restype = None
     _lib = L
@@ -130,6 +130,8 @@ EXPORTED_SYMBOLS = [
     "b200sqp_set_builder",
     "b200sqp_build_instances",
     "b200sqp_download_instances",
+    "b200sqp_default_rollout_settings",
+    "b200sqp_rollout_policy",
     "b200sqp_set_comm",
     "b200sqp_global_stats",
     "b200sqp_global_ladder",

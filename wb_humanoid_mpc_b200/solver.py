@@ -134,11 +134,18 @@ class B200SqpSolver:
         _l.check(_l.lib().b200sqp_upload_instances(self._h, _p(k[0]), _p(k[1]), _p(k[2]), _p(k[3]), k[4].ctypes.data_as(_l.u8p),
                                                    k[5].ctypes.data_as(_l.u8p), _p(k[6]), _p(k[7]), _p(k[8]), _p(k[9])))
 
-    def build_instances(self, t0: float, horizon: float, x0, gaits, gait_start, cmd, warm: bool = False) -> int:
+    def build_instances(self, t0: float, horizon: float, x0, gaits, gait_start, cmd, warm: bool | str = False) -> int:
         """Device-side instance builder (b200sqp_build_instances): one synchronous MPC cycle of len(x0) instances over [t0, t0 + horizon] from
         x0 [B, nx], gait names (or ids) [B], gait start times [B] and velocity commands [B, 4]; warm = shift the iterate left on the device by
-        the previous solve; x0 = None (with warm): the planned state at t0 is the measured state (closed loop on the device).  Returns the common
-        number of shooting nodes."""
+        the previous solve; x0 = None (with warm): the planned state at t0 is the measured state (closed loop on the device); warm = "rollout"
+        (x0 = None): warm start whose measured state is the simulated state of the last rollout_policy.  Returns the common number of shooting
+        nodes."""
+        if warm == "rollout":
+            if x0 is not None:
+                raise ValueError('warm="rollout" takes the measured state from the last roll-out; pass x0=None')
+            warm = 2
+        elif isinstance(warm, str):
+            raise ValueError(f"warm must be a bool or 'rollout', got {warm!r}")
         L = _l.lib()
         if not getattr(self, "_builder_set", False):
             self._bdesc, self._gait_names = abi.builder_desc(self.model)
@@ -183,6 +190,24 @@ class B200SqpSolver:
 
     def wait(self):
         _l.check(_l.lib().b200sqp_wait(self._h))
+
+    def rollout_policy(self, t: float, duration: float, x_start=None, settings: abi.RolloutSettings | None = None, stream=None) -> dict:
+        """MRT_BASE::rolloutPolicy for every instance (b200sqp_rollout_policy): simulate from time t for `duration` seconds under the policy of
+        the last solve (feedback when settings.use_feedback_policy = 1) with the ODE45 roll-out.  x_start [B, nx], or None for the current
+        measured state.  Waits for the result and returns {x [B, nx], u [B, nu], mode [B], n_steps [B, 3] (accepted, rejected, flow-map
+        calls), status [B]}; the simulated state also stays on the device for build_instances(..., warm="rollout")."""
+        B, nx, nu = self.batch, self.nx, self.nu
+        rs = settings if settings is not None else abi.default_rollout_settings()
+        xs = None if x_start is None else _f(x_start)
+        if xs is not None:
+            assert xs.shape == (B, nx), xs.shape
+        out = dict(x=np.zeros((B, nx)), u=np.zeros((B, nu)), mode=np.zeros(B, dtype=np.int32), n_steps=np.zeros((B, 3), dtype=np.int32),
+                   status=np.zeros(B, dtype=np.int32))
+        _l.check(_l.lib().b200sqp_rollout_policy(self._h, C.c_double(t), C.c_double(duration), None if xs is None else _p(xs), C.byref(rs), _p(out["x"]),
+                                                 _p(out["u"]), out["mode"].ctypes.data_as(_l.ip), out["n_steps"].ctypes.data_as(_l.ip),
+                                                 out["status"].ctypes.data_as(_l.ip), C.c_void_p(stream or 0)))
+        self.wait()
+        return out
 
     def run(self, instances):
         batch = stack_instances(instances) if isinstance(instances, list) else instances
