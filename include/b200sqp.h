@@ -215,7 +215,7 @@ int b200sqp_set_builder(b200sqp_handle h, const b200sqp_builder_desc* desc);
  *   simulation of the reference's launch files), which closes the MPC loop without any per-cycle state transfer.
  *   warm = 2: warm start as with warm = 1, the measured state being the simulated state of the last b200sqp_rollout_policy of this batch (x0 must
  *   be NULL; B200SQP_ESTATE without such a roll-out): the closed loop of the reference's dummy simulation (MPC, roll-out, MPC, ...) on the device.
- *   Centroidal handles have no roll-out: warm = 2 returns B200SQP_ESTATE there.
+ *   On a centroidal handle the roll-out is b200sqp_cen_rollout_policy; the padding of the simulated state stays zero.
  * Every instance must produce the same number of shooting nodes (same event count inside the horizon); *n_nodes returns it, B200SQP_EINVAL
  * otherwise (group such instances by gait phase on the host).  Host pointers; ~0.5 kB per instance cross PCIe. */
 int b200sqp_build_instances(b200sqp_handle h, int batch, double t0, double horizon, const double* x0, const int32_t* gait, const double* gait_start,
@@ -268,9 +268,21 @@ void b200sqp_default_rollout_settings(b200sqp_rollout_settings* rs);
  *   input; the reference throws in these cases, here x_end holds the last accepted state).
  * The simulated state stays on the device as the handle's simulated measured state, which b200sqp_build_instances(warm = 2) takes as x0.
  * Like the reference, a t + duration past the plan's last node is not an error: the policy is held at its last node.
- * Needs a finished b200sqp_solve (B200SQP_ESTATE otherwise); whole-body handles only (B200SQP_EINVAL on a centroidal handle). */
+ * Needs a finished b200sqp_solve (B200SQP_ESTATE otherwise).  Whole-body handles only: a centroidal handle returns B200SQP_EINVAL here and
+ * has its own entry point, b200sqp_cen_rollout_policy. */
 int b200sqp_rollout_policy(b200sqp_handle h, double t, double duration, const double* x_start, const b200sqp_rollout_settings* rs, double* x_end,
                            double* u_end, int32_t* mode_end, int32_t* n_steps, int32_t* status, void* stream);
+
+/* The policy roll-out of a centroidal handle (b200sqp_cen_create): CentroidalMpcDummySimNode.cpp:63-76 runs the MRT with
+ * interface.getRollout(), a TimeTriggeredRollout over the OCP's own CentroidalDynamicsAD (CentroidalMpcInterface.cpp:107,231), so the flow map
+ * is the handle's centroidal dynamics (either centroidalModelType).  Same parameters, outputs, errors and asynchrony as b200sqp_rollout_policy,
+ * with x_start / x_end [B][12 + nj]; b200sqp_build_instances(warm = 2) takes its simulated state.  Whole-body handles: B200SQP_EINVAL.
+ * The rollout block of the centroidal task.info (robot_models/unitree_g1/g1_centroidal_mpc/config/mpc/task.info:100-108) differs from the
+ * whole-body one: AbsTolODE 5e-5, RelTolODE 5e-3, timeStep 0.015, maxNumStepsPerSecond 10000 (b200sqp_default_rollout_settings keeps the
+ * whole-body values).  useFeedbackPolicy is false there, so the centroidal dummy loop runs the feed-forward controller by default, and its MRT
+ * runs at 100 Hz against an 80 Hz MPC: one roll-out of 1/100 s per MPC cycle (MRT_ROS_Dummy_Loop.cpp:83). */
+int b200sqp_cen_rollout_policy(b200sqp_handle h, double t, double duration, const double* x_start, const b200sqp_rollout_settings* rs, double* x_end,
+                               double* u_end, int32_t* mode_end, int32_t* n_steps, int32_t* status, void* stream);
 
 /* per-instance iteration record: mirrors sqp::LogEntry / PerformanceIndex (SqpLogging.h, PerformanceIndex.h) */
 typedef struct b200sqp_iter_log {

@@ -9,8 +9,11 @@ gait start, command).  Prints one JSON line.
 WBMpcDummySimNode.cpp) under the new policy with the ODE45 roll-out, and build_instances(warm = 2) takes the simulated state as the next measured
 state; cycles are --mrt-dt apart.  --push S adds a seeded N(0, S) perturbation to the base velocity of the first measured state.  Reports the
 roll-out's host-timed milliseconds per cycle (enqueue to collected results).
---model centroidal: the same loop (perfect tracking) on the centroidal MPC, with the defaults of its task.info (horizon 1.2 s, 80 Hz); also
-reports the builder's milliseconds per cycle and share of the cycle, and the last cycle's stage times (LQ approximation, QP, line search)."""
+--model centroidal: the same loop on the centroidal MPC, with the defaults of its task.info (horizon 1.2 s, 80 Hz); also reports the builder's
+milliseconds per cycle and share of the cycle, and the last cycle's stage times (LQ approximation, QP, line search).  With --sim rollout the
+roll-out is b200sqp_cen_rollout_policy with the centroidal task.info settings, --mrt-dt defaults to 1/100 s (one MRT step of
+CentroidalMpcDummySimNode per MPC cycle), --push perturbs the normalized momentum x[0:6], and the policy is feed-forward unless --feedback is
+given (useFeedbackPolicy false in that task.info)."""
 import argparse
 import json
 import sys
@@ -34,22 +37,27 @@ ap.add_argument("--mpc-dt", type=float, default=None,
                 help="time between MPC cycles; default: mpcDesiredFrequency of the model's task.info (60 Hz whole-body, 80 Hz centroidal)")
 ap.add_argument("--gait", default="walk")
 ap.add_argument("--sim", choices=["tracking", "rollout"], default="tracking")
-ap.add_argument("--mrt-dt", type=float, default=1.0 / 80.0, help="--sim rollout: simulated time per cycle (the MRT step of WBMpcDummySimNode.cpp)")
-ap.add_argument("--push", type=float, default=0.0, help="--sim rollout: std of a seeded perturbation of the first state's base velocity [m/s, rad/s]")
-ap.add_argument("--feedback", type=int, default=1, help="--sim rollout: simulate the linear feedback policy (use_feedback_policy)")
+ap.add_argument("--mrt-dt", type=float, default=None,
+                help="--sim rollout: simulated time per cycle; default: the MRT step of the model's dummy simulation (1/80 s whole-body, 1/100 s centroidal)")
+ap.add_argument("--push", type=float, default=0.0,
+                help="--sim rollout: std of a seeded perturbation of the first state's base velocity [m/s, rad/s] (centroidal: normalized momentum)")
+ap.add_argument("--feedback", type=int, nargs="?", const=1, default=None,
+                help="--sim rollout: simulate the linear feedback policy (use_feedback_policy); default 1 whole-body, 0 centroidal")
 ap.add_argument("--gait-sequence", default=None,
                 help="gait commands as gait@time,... (e.g. stance@0,walk@0.5,run@3,walk@5,stance@7): stateful gait schedule on the device, every "
                      "instance commanded the gait of the current time; replaces --gait")
 args = ap.parse_args()
 cen = args.model == "centroidal"
-if cen and args.sim == "rollout":
-    ap.error("--model centroidal: there is no centroidal policy roll-out; use --sim tracking")
 if cen and args.gait_sequence:
     ap.error("--model centroidal: the stateful gait schedule serves whole-body handles only; use --gait")
 if args.horizon is None:
     args.horizon = 1.2 if cen else 3.5
 if args.mpc_dt is None:
     args.mpc_dt = 1.0 / 80.0 if cen else 1.0 / 60.0
+if args.mrt_dt is None:
+    args.mrt_dt = 1.0 / 100.0 if cen else 1.0 / 80.0
+if args.feedback is None:
+    args.feedback = 0 if cen else 1
 sequence = None
 if args.gait_sequence:
     sequence = [(g, float(t)) for g, t in (item.split("@") for item in args.gait_sequence.split(","))]
@@ -96,8 +104,10 @@ node_counts, ls_ms, ro_ms, ro_bad = {n0}, [], [], 0
 step = args.mrt_dt if rollout else args.mpc_dt
 if rollout:
     xs = x0.copy()
-    xs[:, 29:35] += np.random.default_rng(0).normal(0.0, args.push, (args.batch, 6)) if args.push > 0 else 0.0
-    r = solver.rollout_policy(0.0, step, x_start=xs)   # cycle 0's roll-out (also the warm-up of the kernel)
+    pushed = slice(0, 6) if cen else slice(29, 35)   # normalized momentum / base velocity
+    xs[:, pushed] += np.random.default_rng(0).normal(0.0, args.push, (args.batch, 6)) if args.push > 0 else 0.0
+    rollout_policy = solver.cen_rollout_policy if cen else solver.rollout_policy
+    r = rollout_policy(0.0, step, x_start=xs)   # cycle 0's roll-out (also the warm-up of the kernel)
     ro_bad += int(r["status"].any())
 torch.cuda.synchronize()
 t_begin = time.perf_counter()
@@ -112,7 +122,7 @@ for c in range(1, args.cycles + 1):
     ls_ms.append(solver.benchmarks()[2])
     if rollout:
         t0 = time.perf_counter()
-        r = solver.rollout_policy(c * step, step)
+        r = rollout_policy(c * step, step)
         ro_ms.append(1e3 * (time.perf_counter() - t0))
         ro_bad += int(r["status"].any())
 torch.cuda.synchronize()
@@ -130,7 +140,7 @@ out = {"metric": "SQP solves/sec (G1 whole-body, N=100, batched), receding horiz
 if rollout:
     out.update(sim="rollout", mrt_dt=step, push=args.push, feedback=bool(args.feedback), rollout_ms_per_cycle_median=float(np.median(ro_ms)),
                rollout_ms_per_cycle_mean=float(np.mean(ro_ms)), rollout_steps_last_cycle_median=[float(v) for v in np.median(r["n_steps"], axis=0)],
-               d2h_bytes_per_cycle=12 + int(args.batch * (58 * 8 + 35 * 8 + 5 * 4)))
+               d2h_bytes_per_cycle=12 + int(args.batch * (model["nx"] * 8 + 35 * 8 + 5 * 4)))
 if cen:
     bm = solver.benchmarks()
     out.update(metric=f"SQP solves/sec (G1 centroidal, N={round(args.horizon / model['sqp']['dt'])}, batched), receding horizon on the device", model="centroidal",

@@ -110,6 +110,12 @@ def default_rollout_settings(**over) -> RolloutSettings:
     return s
 
 
+def cen_default_rollout_settings(**over) -> RolloutSettings:
+    """rollout::Settings of the G1 centroidal task.info (ODE45, AbsTolODE 5e-5, RelTolODE 5e-3, timeStep 0.015, maxNumStepsPerSecond 10000), the
+    roll-out of the centroidal dummy simulation (b200sqp_cen_rollout_policy), then keyword overrides."""
+    return default_rollout_settings(**{"abs_tol": 5e-5, "rel_tol": 5e-3, **over})
+
+
 def default_settings(model: dict | None = None, **over) -> Settings:
     """sqp::Settings defaults (SqpSettings.h:42-86) overridden by the G1 task.info values, then by keyword arguments."""
     s = Settings(sqp_iteration=1, delta_tol=1e-4, cost_tol=1e-4, alpha_decay=0.5, alpha_min=1e-4, gamma_c=1e-6, g_max=1e-2, g_min=1e-6,

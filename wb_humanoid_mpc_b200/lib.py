@@ -134,6 +134,7 @@ EXPORTED_SYMBOLS = [
     "b200sqp_download_mode_schedule",
     "b200sqp_default_rollout_settings",
     "b200sqp_rollout_policy",
+    "b200sqp_cen_rollout_policy",
     "b200sqp_set_comm",
     "b200sqp_global_stats",
     "b200sqp_global_ladder",

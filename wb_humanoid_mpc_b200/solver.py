@@ -138,8 +138,9 @@ class B200SqpSolver:
         """Device-side instance builder (b200sqp_build_instances): one synchronous MPC cycle of len(x0) instances over [t0, t0 + horizon] from
         x0 [B, nx], gait names (or ids) [B], gait start times [B] and velocity commands [B, 4]; warm = shift the iterate left on the device by
         the previous solve; x0 = None (with warm): the planned state at t0 is the measured state (closed loop on the device); warm = "rollout"
-        (x0 = None): warm start whose measured state is the simulated state of the last rollout_policy (whole-body handles only).  On a centroidal
-        model x0 is [B, 35] and the targets follow the centroidal rule.  Returns the common number of shooting nodes."""
+        (x0 = None): warm start whose measured state is the simulated state of the last roll-out (rollout_policy on a whole-body model,
+        cen_rollout_policy on a centroidal one).  On a centroidal model x0 is [B, 35] and the targets follow the centroidal rule.  Returns the
+        common number of shooting nodes."""
         if warm == "rollout":
             if x0 is not None:
                 raise ValueError('warm="rollout" takes the measured state from the last roll-out; pass x0=None')
@@ -209,16 +210,23 @@ class B200SqpSolver:
         the last solve (feedback when settings.use_feedback_policy = 1) with the ODE45 roll-out.  x_start [B, nx], or None for the current
         measured state.  Waits for the result and returns {x [B, nx], u [B, nu], mode [B], n_steps [B, 3] (accepted, rejected, flow-map
         calls), status [B]}; the simulated state also stays on the device for build_instances(..., warm="rollout")."""
+        return self._rollout(_l.lib().b200sqp_rollout_policy, t, duration, x_start, settings if settings is not None else abi.default_rollout_settings(), stream)
+
+    def cen_rollout_policy(self, t: float, duration: float, x_start=None, settings: abi.RolloutSettings | None = None, stream=None) -> dict:
+        """rollout_policy on a centroidal model (b200sqp_cen_rollout_policy): the ODE45 roll-out of the centroidal flow map under the policy of
+        the last solve, by default with the centroidal task.info settings (abi.cen_default_rollout_settings).  x_start [B, 35] or None; returns
+        the dict of rollout_policy with x [B, 35]; the simulated state stays on the device for build_instances(..., warm="rollout")."""
+        return self._rollout(_l.lib().b200sqp_cen_rollout_policy, t, duration, x_start, settings if settings is not None else abi.cen_default_rollout_settings(), stream)
+
+    def _rollout(self, fn, t, duration, x_start, rs, stream):
         B, nx, nu = self.batch, self.nx, self.nu
-        rs = settings if settings is not None else abi.default_rollout_settings()
         xs = None if x_start is None else _f(x_start)
         if xs is not None:
             assert xs.shape == (B, nx), xs.shape
         out = dict(x=np.zeros((B, nx)), u=np.zeros((B, nu)), mode=np.zeros(B, dtype=np.int32), n_steps=np.zeros((B, 3), dtype=np.int32),
                    status=np.zeros(B, dtype=np.int32))
-        _l.check(_l.lib().b200sqp_rollout_policy(self._h, C.c_double(t), C.c_double(duration), None if xs is None else _p(xs), C.byref(rs), _p(out["x"]),
-                                                 _p(out["u"]), out["mode"].ctypes.data_as(_l.ip), out["n_steps"].ctypes.data_as(_l.ip),
-                                                 out["status"].ctypes.data_as(_l.ip), C.c_void_p(stream or 0)))
+        _l.check(fn(self._h, C.c_double(t), C.c_double(duration), None if xs is None else _p(xs), C.byref(rs), _p(out["x"]), _p(out["u"]),
+                    out["mode"].ctypes.data_as(_l.ip), out["n_steps"].ctypes.data_as(_l.ip), out["status"].ctypes.data_as(_l.ip), C.c_void_p(stream or 0)))
         self.wait()
         return out
 
