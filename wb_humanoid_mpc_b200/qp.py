@@ -59,14 +59,18 @@ class BatchedQp:
         _l.check(_l.lib().b200sqp_qp_last_ms(self._h, C.byref(ms)))
         return ms.value
 
-    def download(self):
+    def download(self, raise_on_failure: bool = True):
+        """A failed factorisation of some instance raises (B200SqpError -4) unless raise_on_failure = False, in which case the dict is returned
+        with the per-instance `status` array (the arrays of the other instances are valid either way)."""
         Bn, N, nx, nm = self.batch, self.N, self.nx, self.nu_max
         dx, du = np.zeros((Bn, N + 1, nx)), np.zeros((Bn, N, nm))
         K, k = np.zeros((Bn, N, nx, nm)), np.zeros((Bn, N, nm))
         P = np.zeros((Bn, N + 1, nx, nx)) if self._keptP else None
         p = np.zeros((Bn, N + 1, nx)) if self._keptP else None
         status = np.zeros(Bn, dtype=np.int32)
-        _l.check(_l.lib().b200sqp_qp_download(self._h, _p(dx), _p(du), _p(K), _p(k), _p(P), _p(p), status.ctypes.data_as(_l.ip)))
+        rc = _l.lib().b200sqp_qp_download(self._h, _p(dx), _p(du), _p(K), _p(k), _p(P), _p(p), status.ctypes.data_as(_l.ip))
+        if rc != 0 and (raise_on_failure or rc != -4):   # -4 = B200SQP_EQP: every array has been filled, status says which instances failed
+            _l.check(rc)
         out = dict(dx=dx, du=du, K=np.swapaxes(K, -1, -2).copy(), k=k, status=status)
         if self._keptP:
             out["P"] = np.swapaxes(P, -1, -2).copy()
