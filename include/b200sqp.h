@@ -567,6 +567,45 @@ int b200sqp_fleet_command_poses(b200sqp_fleet f, int count, const int32_t* insta
 int b200sqp_fleet_clear_poses(b200sqp_fleet f, int count, const int32_t* instances);
 int b200sqp_fleet_download_pose_targets(b200sqp_fleet f, int32_t* active, double* t_start, double* t_reach, double* target_pose, double* error);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Device-pointer I/O: the boundary of the closed loop in GPU memory, for a batched simulator whose robot states already live on the device.
+ * Every pointer argument below is device (or managed) memory on the handle's device, except gait, gait_start, cmd, n_nodes and n_groups,
+ * which are host arrays as in the host entry points.  Each device pointer is checked with cudaPointerGetAttributes: anything else returns
+ * B200SQP_EINVAL and enqueues nothing.  `stream` is a cudaStream_t (NULL: the legacy default stream).
+ *
+ * b200sqp_build_instances_dev / b200sqp_fleet_build_instances_dev: b200sqp_build_instances / b200sqp_fleet_build_instances with the measured
+ *   states x0_dev [B][nx] (35 wide on centroidal handles) in device memory; x0_dev is required (x0 = NULL builds use the host entry points)
+ *   and warm is 0 or 1 (warm = 2 takes the simulated state: B200SQP_EINVAL).  The build reads x0_dev after the work enqueued on `stream`
+ *   before the call (a producer kernel of the caller is seen).  Everything else, synchronisation and return codes included, is the host build.
+ * b200sqp_joint_actions_dev / b200sqp_fleet_joint_actions_dev: b200sqp_joint_actions with robot_state_dev [B][13 + 2 nj] in device memory
+ *   (NULL: the end state of the last roll-out) and every output in device memory (each may be NULL).  The call enqueues its work on `stream`
+ *   and returns: no host synchronisation, no pageable copy, no allocation after the first call at a batch size.  The robot-state check of
+ *   the host entry point (every entry finite, |quaternion norm - 1| <= 1e-6) runs on the device per row and writes status [B] (may be NULL):
+ *   0 accepted, 1 an entry is not finite, 2 the quaternion norm is off.  A rejected row gets NaN in every double output and mode -1; every
+ *   other row is bit-identical to what b200sqp_joint_actions returns for it.  B200SQP_EINVAL (t, use_policy) and B200SQP_ESTATE (no batch,
+ *   solve or roll-out) as on the host path.
+ * b200sqp_download_dev / b200sqp_fleet_download_dev: the x, u, K and status outputs of b200sqp_download / b200sqp_fleet_download (caller order,
+ *   fleets padded to max_nodes rows with zeros, centroidal rows 35 wide), enqueued on `stream`; each may be NULL.  status [B] is the
+ *   per-instance solve status: the call cannot see it without a synchronisation, so it returns 0 where the host download returns
+ *   B200SQP_EQP.  K needs settings.use_feedback_policy (B200SQP_ESTATE).  n_nodes [B] (fleet, host, may be NULL): each instance's node count.
+ *
+ * Ordering: calls on one handle run on the device in the order they were made, whatever streams they are given.  A _dev call enqueues behind
+ *   the handle's outstanding work (a solve or roll-out in flight, the last _dev call) with stream waits, not host waits, and records an event
+ *   after its own work; every entry point that touches what a _dev call reads or writes (the plan, the simulated state, the joint-action
+ *   scratch, the fleet carry) makes its stream wait on that event before it enqueues anything, and memory is not freed under it.
+ *   b200sqp_wait / b200sqp_fleet_wait also wait for outstanding _dev work.  When no _dev call was made, nothing new is recorded or waited on.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int b200sqp_build_instances_dev(b200sqp_handle h, int batch, double t0, double horizon, const double* x0_dev, const int32_t* gait,
+                                const double* gait_start, const double* cmd, int warm, int32_t* n_nodes, void* stream);
+int b200sqp_fleet_build_instances_dev(b200sqp_fleet f, int batch, double t0, double horizon, const double* x0_dev, const int32_t* gait,
+                                      const double* gait_start, const double* cmd, int warm, int32_t* n_nodes, int32_t* n_groups, void* stream);
+int b200sqp_joint_actions_dev(b200sqp_handle h, double t, const double* robot_state_dev, int use_policy, double* q_des, double* qd_des, double* tau_ff,
+                              double* x_obs, double* u_policy, int32_t* mode, int32_t* status, void* stream);
+int b200sqp_fleet_joint_actions_dev(b200sqp_fleet f, double t, const double* robot_state_dev, int use_policy, double* q_des, double* qd_des,
+                                    double* tau_ff, double* x_obs, double* u_policy, int32_t* mode, int32_t* status, void* stream);
+int b200sqp_download_dev(b200sqp_handle h, double* x, double* u, double* K, int32_t* status, void* stream);
+int b200sqp_fleet_download_dev(b200sqp_fleet f, int max_nodes, double* x, double* u, double* K, int32_t* status, int32_t* n_nodes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -178,4 +178,10 @@ EXPORTED_SYMBOLS = [
     "b200sqp_fleet_command_poses",
     "b200sqp_fleet_clear_poses",
     "b200sqp_fleet_download_pose_targets",
+    "b200sqp_build_instances_dev",
+    "b200sqp_fleet_build_instances_dev",
+    "b200sqp_joint_actions_dev",
+    "b200sqp_fleet_joint_actions_dev",
+    "b200sqp_download_dev",
+    "b200sqp_fleet_download_dev",
 ]

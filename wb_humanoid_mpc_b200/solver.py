@@ -80,6 +80,62 @@ def _pose_targets(fn, h, B):
     return dict(active=act.astype(bool), t_start=ts, t_reach=tr, target_pose=tp, error=err)
 
 
+def _is_cuda_tensor(a) -> bool:
+    return getattr(a, "is_cuda", False) is True
+
+
+def check_device_tensor(t, name: str, device, dtype, shape):
+    """The checks of a device-pointer argument, before any ABI call: a torch tensor on `device` of `dtype`, with `shape`, C-contiguous.
+    Raises ValueError naming the argument."""
+    import torch
+
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{name}: expected a torch tensor, got {type(t).__name__}")
+    if t.device != torch.device(device):
+        raise ValueError(f"{name}: the tensor is on {t.device}, the handle on {torch.device(device)}")
+    if t.dtype != dtype:
+        raise ValueError(f"{name}: dtype {t.dtype}, expected {dtype}")
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{name}: shape {tuple(t.shape)}, expected {tuple(shape)}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name}: the tensor is not C-contiguous")
+    return t
+
+
+def _vp(t):
+    return C.c_void_p(None if t is None else t.data_ptr())
+
+
+def _stream(device, stream) -> C.c_void_p:
+    """stream = None: the current torch stream of the handle's device; a torch.cuda.Stream or a raw cudaStream_t (int) otherwise"""
+    import torch
+
+    if stream is None:
+        stream = torch.cuda.current_stream(device)
+    return C.c_void_p(getattr(stream, "cuda_stream", stream) or 0)
+
+
+def _device_outputs(device, specs: dict, out: dict | None) -> dict:
+    """specs {name: (shape, dtype)} -> the caller's tensors (checked) or new ones"""
+    import torch
+
+    if out is None:
+        return {k: torch.empty(shape, dtype=dt, device=device) for k, (shape, dt) in specs.items()}
+    return {k: check_device_tensor(out.get(k), f"out[{k!r}]", device, dt, shape) for k, (shape, dt) in specs.items()}
+
+
+def _joint_actions_device(fn, h, device, B, nx, nu, nj, t, robot_state, use_policy, out, stream) -> dict:
+    import torch
+
+    rs = None if robot_state is None else check_device_tensor(robot_state, "robot_state", device, torch.float64, (B, 13 + 2 * nj))
+    f64, i32 = torch.float64, torch.int32
+    o = _device_outputs(device, dict(q_des=((B, nj), f64), qd_des=((B, nj), f64), tau=((B, nj), f64), x=((B, nx), f64), u=((B, nu), f64),
+                                     mode=((B,), i32), status=((B,), i32)), out)
+    _l.check(fn(h, C.c_double(t), _vp(rs), C.c_int(int(use_policy)), _vp(o["q_des"]), _vp(o["qd_des"]), _vp(o["tau"]), _vp(o["x"]), _vp(o["u"]),
+                _vp(o["mode"]), _vp(o["status"]), _stream(device, stream)))
+    return o
+
+
 def stack_instances(instances: list[dict]) -> dict:
     """list of per-instance dicts (references.build_instance) -> batched arrays; all instances must share the node count."""
     n = {len(i["t_nodes"]) for i in instances}
@@ -108,6 +164,7 @@ class B200SqpSolver:
             _l.check(L.b200sqp_stage_doubles(self._h, C.c_int(0), C.byref(per)))
             self._raw_per = per.value
         self.batch = self.n_nodes = 0
+        self.device = device
         self._nccl = self._comm = None
 
     # -- global-step mode (SURVEY.md section 8e) --------------------------------------------------------------------------------
@@ -195,7 +252,10 @@ class B200SqpSolver:
         (x0 = None): warm start whose measured state is the simulated state of the last roll-out (rollout_policy on a whole-body model,
         cen_rollout_policy on a centroidal one).  On a centroidal model x0 is [B, 35] and the targets follow the centroidal rule.  Returns the
         common number of shooting nodes.  With a motion manager (set_motion_manager) cmd is the raw velocity command and gaits may be None on
-        warm builds."""
+        warm builds.  x0 may be a float64 CUDA tensor on the handle's device (b200sqp_build_instances_dev): the build reads it after the work
+        enqueued so far on the current torch stream."""
+        if _is_cuda_tensor(x0):
+            return self._build_dev(t0, horizon, x0, gaits, gait_start, cmd, warm)
         if warm == "rollout":
             if x0 is not None:
                 raise ValueError('warm="rollout" takes the measured state from the last roll-out; pass x0=None')
@@ -209,6 +269,21 @@ class B200SqpSolver:
         n = C.c_int32()
         _l.check(L.b200sqp_build_instances(self._h, C.c_int(B), C.c_double(t0), C.c_double(horizon), None if x0 is None else _p(x0),
                                            None if gid is None else gid.ctypes.data_as(_l.ip), _p(gs), _p(cm), C.c_int(int(warm)), C.byref(n)))
+        self.batch, self.n_nodes = B, n.value
+        return n.value
+
+    def _build_dev(self, t0, horizon, x0, gaits, gait_start, cmd, warm):
+        import torch
+
+        if isinstance(warm, str):
+            raise ValueError(f"warm must be a bool with a device x0 (warm='rollout' takes the simulated state), got {warm!r}")
+        self._ensure_builder()
+        B, gid, gs, cm = _build_args(None, gaits, gait_start, cmd, self._gait_names)
+        check_device_tensor(x0, "x0", torch.device("cuda", self.device), torch.float64, (B, self.nx))
+        n = C.c_int32()
+        _l.check(_l.lib().b200sqp_build_instances_dev(self._h, C.c_int(B), C.c_double(t0), C.c_double(horizon), _vp(x0),
+                                                      None if gid is None else gid.ctypes.data_as(_l.ip), _p(gs), _p(cm), C.c_int(int(warm)), C.byref(n),
+                                                      _stream(torch.device("cuda", self.device), None)))
         self.batch, self.n_nodes = B, n.value
         return n.value
 
@@ -358,6 +433,31 @@ class B200SqpSolver:
         self.wait()
         return out
 
+    def joint_actions_device(self, t: float, robot_state=None, use_policy: bool = True, out: dict | None = None, stream=None) -> dict:
+        """joint_actions in device memory (b200sqp_joint_actions_dev): robot_state a float64 CUDA tensor [B, 13 + 2 nj] on the handle's device,
+        or None for the end state of the last roll-out.  Enqueued on `stream` (default: the current torch stream) without waiting; returns CUDA
+        tensors {q_des, qd_des, tau [B, nj], x [B, nx], u [B, nu], mode [B], status [B]} (int32 mode / status), or fills `out`, a dict of such
+        tensors.  status: 0 accepted, 1 a non-finite entry, 2 a quaternion norm off 1 by more than 1e-6; a rejected row gets NaN and mode -1."""
+        import torch
+
+        return _joint_actions_device(_l.lib().b200sqp_joint_actions_dev, self._h, torch.device("cuda", self.device), self.batch, self.nx, self.nu,
+                                     self.model["nj"], t, robot_state, use_policy, out, stream)
+
+    def primal_solution_device(self, with_gains: bool | None = None, stream=None) -> dict:
+        """primal_solution in device memory (b200sqp_download_dev), enqueued on `stream` without waiting: CUDA tensors {x [B, n, nx],
+        u [B, n-1, nu], status [B] (int32, the per-instance solve status; nothing is raised), K [B, n-1, nu, nx] (a transposed view) with gains}"""
+        import torch
+
+        dev = torch.device("cuda", self.device)
+        B, n, nx, nu = self.batch, self.n_nodes, self.nx, self.nu
+        with_gains = bool(self.settings.use_feedback_policy) if with_gains is None else with_gains
+        o = _device_outputs(dev, dict(x=((B, n, nx), torch.float64), u=((B, n - 1, nu), torch.float64), status=((B,), torch.int32)), None)
+        K = torch.empty((B, n - 1, nx, nu), dtype=torch.float64, device=dev) if with_gains else None
+        _l.check(_l.lib().b200sqp_download_dev(self._h, _vp(o["x"]), _vp(o["u"]), _vp(K), _vp(o["status"]), _stream(dev, stream)))
+        if K is not None:
+            o["K"] = K.transpose(-1, -2)
+        return o
+
     def _rollout(self, fn, t, duration, x_start, rs, stream):
         B, nx, nu = self.batch, self.nx, self.nu
         xs = None if x_start is None else _f(x_start)
@@ -473,7 +573,10 @@ class B200SqpFleet:
             pass
 
     def build_instances(self, t0: float, horizon: float, x0, gaits, gait_start, cmd, warm: bool | str = False) -> np.ndarray:
-        """B200SqpSolver.build_instances for instances of any node count; returns n_nodes [B] (self.n_groups: the distinct counts)"""
+        """B200SqpSolver.build_instances for instances of any node count; returns n_nodes [B] (self.n_groups: the distinct counts).  x0 may be a
+        float64 CUDA tensor (b200sqp_fleet_build_instances_dev)."""
+        if _is_cuda_tensor(x0):
+            return self._build_dev(t0, horizon, x0, gaits, gait_start, cmd, warm)
         if warm == "rollout":
             if x0 is not None:
                 raise ValueError('warm="rollout" takes the measured state from the last roll-out; pass x0=None')
@@ -486,6 +589,21 @@ class B200SqpFleet:
         _l.check(_l.lib().b200sqp_fleet_build_instances(self._f, C.c_int(B), C.c_double(t0), C.c_double(horizon), None if x0 is None else _p(x0),
                                                         None if gid is None else gid.ctypes.data_as(_l.ip), _p(gs), _p(cm), C.c_int(int(warm)),
                                                         n.ctypes.data_as(_l.ip), C.byref(G)))
+        self.batch, self.n_nodes, self.n_groups = B, n, G.value
+        return n.copy()
+
+    def _build_dev(self, t0, horizon, x0, gaits, gait_start, cmd, warm):
+        import torch
+
+        if isinstance(warm, str):
+            raise ValueError(f"warm must be a bool with a device x0 (warm='rollout' takes the simulated state), got {warm!r}")
+        dev = torch.device("cuda", self.solver.device)
+        B, gid, gs, cm = _build_args(None, gaits, gait_start, cmd, self.solver._gait_names)
+        check_device_tensor(x0, "x0", dev, torch.float64, (B, self.nx))
+        n, G = np.zeros(B, dtype=np.int32), C.c_int32()
+        _l.check(_l.lib().b200sqp_fleet_build_instances_dev(self._f, C.c_int(B), C.c_double(t0), C.c_double(horizon), _vp(x0),
+                                                            None if gid is None else gid.ctypes.data_as(_l.ip), _p(gs), _p(cm), C.c_int(int(warm)),
+                                                            n.ctypes.data_as(_l.ip), C.byref(G), _stream(dev, None)))
         self.batch, self.n_nodes, self.n_groups = B, n, G.value
         return n.copy()
 
@@ -590,6 +708,31 @@ class B200SqpFleet:
                                                       C.c_void_p(stream or 0)))
         self.wait()
         return out
+
+    def joint_actions_device(self, t: float, robot_state=None, use_policy: bool = True, out: dict | None = None, stream=None) -> dict:
+        """B200SqpSolver.joint_actions_device (b200sqp_fleet_joint_actions_dev), caller order"""
+        import torch
+
+        return _joint_actions_device(_l.lib().b200sqp_fleet_joint_actions_dev, self._f, torch.device("cuda", self.solver.device), self.batch, self.nx,
+                                     self.nu, self.model["nj"], t, robot_state, use_policy, out, stream)
+
+    def primal_solution_device(self, with_gains: bool | None = None, stream=None) -> dict:
+        """B200SqpSolver.primal_solution_device (b200sqp_fleet_download_dev): x [B, m, nx], u [B, m - 1, nu] (m = max(n_nodes), rows past an
+        instance's n_nodes zero), status, K with gains, as CUDA tensors, and n_nodes [B] (numpy)"""
+        import torch
+
+        dev = torch.device("cuda", self.solver.device)
+        B, m, nx, nu = self.batch, int(self.n_nodes.max()), self.nx, self.nu
+        with_gains = bool(self.settings.use_feedback_policy) if with_gains is None else with_gains
+        o = _device_outputs(dev, dict(x=((B, m, nx), torch.float64), u=((B, m - 1, nu), torch.float64), status=((B,), torch.int32)), None)
+        K = torch.empty((B, m - 1, nx, nu), dtype=torch.float64, device=dev) if with_gains else None
+        n_nodes = np.zeros(B, dtype=np.int32)
+        _l.check(_l.lib().b200sqp_fleet_download_dev(self._f, C.c_int(m), _vp(o["x"]), _vp(o["u"]), _vp(K), _vp(o["status"]), n_nodes.ctypes.data_as(_l.ip),
+                                                     _stream(dev, stream)))
+        if K is not None:
+            o["K"] = K.transpose(-1, -2)
+        o["n_nodes"] = n_nodes
+        return o
 
     def benchmarks(self):
         """device milliseconds of {LQ approximation, solve QP, line search, projection} of the last solve, summed over its groups"""
