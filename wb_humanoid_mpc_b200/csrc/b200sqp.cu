@@ -12,6 +12,7 @@
 #include <memory>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "riccati.cuh"
@@ -106,7 +107,65 @@ int launch_riccati(const b200sqp::QpDeviceView& v, cudaStream_t st) {
   }
   return 1;
 }
+
+// a failed allocation, reported as the error of the entry point that made it
+int failAlloc(const char* entry, cudaError_t e) {
+  return fail(e == cudaErrorMemoryAllocation ? B200SQP_ENOMEM : B200SQP_ENODEV, "%s: %s", entry, cudaGetErrorString(e));
+}
 }  // namespace
+
+namespace b200sqp {
+// The device and pinned allocations of one lifetime.  Each allocation stores its pointer in a field of the caller and records that field;
+// release(from) frees what was allocated since mark() returned `from`, newest first, and sets each recorded field back to null.  The first
+// error is sticky -- later allocations do nothing, so a group of them is checked once with error() -- until release() clears it.
+class MemOwner {
+ public:
+  MemOwner() = default;
+  MemOwner(const MemOwner&) = delete;
+  MemOwner& operator=(const MemOwner&) = delete;
+  ~MemOwner() { release(); }
+  template <class T>
+  void device(T*& field, size_t count, bool zero = false) {
+    add(slot(field), count * sizeof(T), false, zero);
+  }
+  template <class T>
+  void pinned(T*& field, size_t count) {
+    add(slot(field), count * sizeof(T), true, false);
+  }
+  cudaError_t error() const { return err_; }
+  size_t mark() const { return live_.size(); }
+  void release(size_t from = 0) {
+    for (; live_.size() > from; live_.pop_back()) {
+      void** field = live_.back().field;
+      if (live_.back().pinned) cudaFreeHost(*field);
+      else cudaFree(*field);
+      *field = nullptr;
+    }
+    err_ = cudaSuccess;
+  }
+
+ private:
+  struct Entry {
+    void** field;
+    bool pinned;
+  };
+  template <class T>
+  static void** slot(T*& field) {   // (const-qualified T: the device arrays a kernel only reads)
+    return reinterpret_cast<void**>(const_cast<std::remove_const_t<T>**>(&field));
+  }
+  void add(void** field, size_t bytes, bool pinned, bool zero) {
+    if (err_ != cudaSuccess) return;
+    void* p = nullptr;
+    err_ = pinned ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes);
+    if (err_ != cudaSuccess) return;
+    *field = p;
+    live_.push_back({field, pinned});
+    if (zero) err_ = cudaMemset(p, 0, bytes);
+  }
+  std::vector<Entry> live_;
+  cudaError_t err_ = cudaSuccess;
+};
+}  // namespace b200sqp
 
 struct b200sqp_qp_t {
   int device = 0, B = 0, N = 0, nx = 0, numax = 0;
@@ -117,6 +176,7 @@ struct b200sqp_qp_t {
   int* status = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   bool uploaded = false, solved = false, keptP = false;
+  b200sqp::MemOwner mem;
 };
 
 extern "C" {
@@ -138,33 +198,31 @@ int b200sqp_qp_create(int device, int batch, int N, int nx, int nu_max, b200sqp_
   qp->nx = nx;
   qp->numax = nu_max;
   const size_t bn = static_cast<size_t>(batch) * N, bn1 = static_cast<size_t>(batch) * (N + 1);
-  auto alloc = [&](double** p, size_t n) { return cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(double)); };
-  cudaError_t e = cudaSuccess;
-  auto A_ = [&](cudaError_t r) { if (e == cudaSuccess) e = r; };
-  A_(alloc(&qp->A, bn * nx * nx));
-  A_(alloc(&qp->Bm, bn * nx * nu_max));
-  A_(alloc(&qp->b, bn * nx));
-  A_(alloc(&qp->Q, bn1 * nx * nx));
-  A_(alloc(&qp->S, bn * nu_max * nx));
-  A_(alloc(&qp->R, bn * nu_max * nu_max));
-  A_(alloc(&qp->q, bn1 * nx));
-  A_(alloc(&qp->r, bn * nu_max));
-  A_(alloc(&qp->dx0, static_cast<size_t>(batch) * nx));
-  A_(cudaMalloc(reinterpret_cast<void**>(&qp->nu), bn * sizeof(int)));
-  A_(alloc(&qp->K, bn * nu_max * nx));
-  A_(alloc(&qp->kff, bn * nu_max));
-  A_(alloc(&qp->P, bn1 * nx * nx));
-  A_(alloc(&qp->p, bn1 * nx));
-  A_(alloc(&qp->dx, bn1 * nx));
-  A_(alloc(&qp->du, bn * nu_max));
-  A_(cudaMalloc(reinterpret_cast<void**>(&qp->status), batch * sizeof(int)));
-  A_(cudaEventCreate(&qp->ev0));
-  A_(cudaEventCreate(&qp->ev1));
-  if (e == cudaSuccess)
-    e = set_riccati_smem_attributes(nx, nu_max);
+  b200sqp::MemOwner& m = qp->mem;
+  m.device(qp->A, bn * nx * nx);
+  m.device(qp->Bm, bn * nx * nu_max);
+  m.device(qp->b, bn * nx);
+  m.device(qp->Q, bn1 * nx * nx);
+  m.device(qp->S, bn * nu_max * nx);
+  m.device(qp->R, bn * nu_max * nu_max);
+  m.device(qp->q, bn1 * nx);
+  m.device(qp->r, bn * nu_max);
+  m.device(qp->dx0, static_cast<size_t>(batch) * nx);
+  m.device(qp->nu, bn);
+  m.device(qp->K, bn * nu_max * nx);
+  m.device(qp->kff, bn * nu_max);
+  m.device(qp->P, bn1 * nx * nx);
+  m.device(qp->p, bn1 * nx);
+  m.device(qp->dx, bn1 * nx);
+  m.device(qp->du, bn * nu_max);
+  m.device(qp->status, batch);
+  cudaError_t e = m.error();
+  if (e == cudaSuccess) e = cudaEventCreate(&qp->ev0);
+  if (e == cudaSuccess) e = cudaEventCreate(&qp->ev1);
+  if (e == cudaSuccess) e = set_riccati_smem_attributes(nx, nu_max);
   if (e != cudaSuccess) {
     b200sqp_qp_destroy(qp);
-    return fail(e == cudaErrorMemoryAllocation ? B200SQP_ENOMEM : B200SQP_ENODEV, "qp_create: %s", cudaGetErrorString(e));
+    return failAlloc("qp_create", e);
   }
   *out = qp;
   return 0;
@@ -173,13 +231,9 @@ int b200sqp_qp_create(int device, int batch, int N, int nx, int nu_max, b200sqp_
 void b200sqp_qp_destroy(b200sqp_qp qp) {
   if (!qp) return;
   cudaSetDevice(qp->device);
-  for (double* p : {qp->A, qp->Bm, qp->b, qp->Q, qp->S, qp->R, qp->q, qp->r, qp->dx0, qp->K, qp->kff, qp->P, qp->p, qp->dx, qp->du})
-    if (p) cudaFree(p);
-  if (qp->nu) cudaFree(qp->nu);
-  if (qp->status) cudaFree(qp->status);
   if (qp->ev0) cudaEventDestroy(qp->ev0);
   if (qp->ev1) cudaEventDestroy(qp->ev1);
-  delete qp;
+  delete qp;   // (its owner frees the arrays)
 }
 
 int b200sqp_qp_upload(b200sqp_qp qp, const double* A, const double* B, const double* b, const double* Q, const double* S,
