@@ -11,7 +11,6 @@
 #ifdef EMU_WITH_LQ
 #include "../../wb_humanoid_mpc_b200/csrc/wb_lq.cuh"
 #include "../../wb_humanoid_mpc_b200/csrc/cen_host.cuh"
-#include "../../wb_humanoid_mpc_b200/csrc/wb_builder.cuh"
 #endif
 
 using namespace b200sqp;
@@ -63,6 +62,5 @@ int emu_joint_torques(const b200sqp_model_desc* d, const double* x, const double
 #ifdef EMU_WITH_LQ
 #include "wb_emu_lq.inc"
 #include "cen_emu.inc"
-#include "builder_emu.inc"
 #endif
 }

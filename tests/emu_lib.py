@@ -3,34 +3,19 @@ executed on the host.  Test infrastructure only -- never linked into or called b
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
+from emu_build import build
 from oracle_lib import F, _p, unpack_raw_blocks
 
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "emu"
-CSRC = ROOT / "wb_humanoid_mpc_b200" / "csrc"
 _lib = None
-
-
-def build(force=False):
-    so = EMU / "libwbemu.so"
-    srcs = list(EMU.glob("*.cu")) + list(EMU.glob("*.inc")) + list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.inc"))
-    if force or not so.exists() or any(s.stat().st_mtime > so.stat().st_mtime for s in srcs):
-        nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-        subprocess.run([nvcc, "-O2", "-std=c++17", "-DEMU_WITH_LQ", "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC", "-Wno-deprecated-gpu-targets",
-                        "-diag-suppress", "177", "-o", str(so), str(EMU / "wb_emu.cu")], check=True)
-    return so
 
 
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(str(build()))
+        _lib = C.CDLL(str(build("wb_emu.cu", "libwbemu.so", defines=["EMU_WITH_LQ"], deps=["wb_emu_lq.inc", "cen_emu.inc"])))
     return _lib
 
 
@@ -95,43 +80,3 @@ def joint_torques(desc, x, u):
     assert rc == 0
     return tau, qddb
 
-
-def build_instances(model, t0, horizon, x0, gaits, gait_start, cmd, previous=None, cap=None):
-    """the device-side instance builder (wb_builder.cuh) on the CPU harness -> dict in the layout of solver.stack_instances, or a negative error code.
-    previous = dict(t [B, n], event [B, n], x [B, n, nx], u [B, n-1, nu]) enables the warm start."""
-    from wb_humanoid_mpc_b200 import abi
-
-    desc, names = abi.builder_desc(model)
-    x0 = F(x0)
-    B, nx, nu = x0.shape[0], model["nx"], model["nu"]
-    gid = np.ascontiguousarray([names.index(g) for g in gaits], dtype=np.int32)
-    gs, cm = F(gait_start), F(cmd)
-    cap = cap or int(horizon / desc.dt) + 2 + 96
-    out = dict(x_init=np.zeros((B, cap, nx)), u_init=np.zeros((B, cap, nu)), t_nodes=np.zeros((B, cap)), node_event=np.zeros((B, cap), dtype=np.uint8),
-               contact_flags=np.zeros((B, cap, 2), dtype=np.uint8), swing_ref=np.zeros((B, cap, 2, 3)), impact_factor=np.zeros((B, cap, 2)),
-               arm_phase=np.zeros((B, cap)), x_ref=np.zeros((B, cap, nx)))
-    u8p = C.POINTER(C.c_uint8)
-    ip = C.POINTER(C.c_int32)
-    if previous is not None:
-        pT, pE, pX, pU = F(previous["t"]), np.ascontiguousarray(previous["event"], dtype=np.uint8), F(previous["x"]), F(previous["u"])
-        prevN = pT.shape[1] - 1
-        pa = (_p(pT), pE.ctypes.data_as(u8p), _p(pX), _p(pU))
-    else:
-        prevN, pa = 0, (None, None, None, None)
-    L = lib()
-    L.emu_build_instances.restype = C.c_int
-    n = L.emu_build_instances(C.byref(desc), C.c_int(B), C.c_double(t0), C.c_double(horizon), _p(x0), gid.ctypes.data_as(ip), _p(gs), _p(cm),
-                              C.c_int(int(previous is not None)), C.c_int(prevN), *pa, C.c_int(cap), _p(out["x_init"]), _p(out["u_init"]), _p(out["t_nodes"]),
-                              out["node_event"].ctypes.data_as(u8p), out["contact_flags"].ctypes.data_as(u8p), _p(out["swing_ref"]), _p(out["impact_factor"]),
-                              _p(out["arm_phase"]), _p(out["x_ref"]))
-    if n < 0:
-        return n
-    # the harness writes with the strides of the actual node count
-    res = {}
-    for k, v in out.items():
-        per = int(np.prod(v.shape[2:])) if v.ndim > 2 else 1
-        rows = n - 1 if k == "u_init" else n
-        flat = v.reshape(-1)[: B * rows * per]
-        res[k] = flat.reshape((B, rows) + v.shape[2:]).copy()
-    res["x0"] = x0
-    return res

@@ -4,35 +4,20 @@ library."""
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
+from emu_build import build
 from oracle_lib import F, _p
 
-ROOT = Path(__file__).resolve().parents[1]
-EMU = ROOT / "tests" / "emu"
-CSRC = ROOT / "wb_humanoid_mpc_b200" / "csrc"
 NX, NU, NJ = 58, 35, 23
 _lib = None
-
-
-def build(force=False):
-    so = EMU / "libmrtemu.so"
-    srcs = [EMU / "mrt_emu.cu"] + list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.inc")) + [ROOT / "include" / "b200sqp.h"]
-    if force or not so.exists() or any(s.stat().st_mtime > so.stat().st_mtime for s in srcs):
-        nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-        subprocess.run([nvcc, "-O2", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC", "-Wno-deprecated-gpu-targets",
-                        "-diag-suppress", "177", "-o", str(so), str(EMU / "mrt_emu.cu")], check=True)
-    return so
 
 
 def lib():
     global _lib
     if _lib is None:
-        _lib = C.CDLL(str(build()))
+        _lib = C.CDLL(str(build("mrt_emu.cu", "libmrtemu.so")))
     return _lib
 
 

@@ -7,7 +7,7 @@ import math
 import numpy as np
 import pytest
 
-import cen_motion_emu_lib as E
+import bld_emu_lib as E
 import oracle_lib as orc
 from wb_humanoid_mpc_b200 import abi, centroidal, host_lib, model_loader
 from wb_humanoid_mpc_b200 import references as R
@@ -122,7 +122,7 @@ def test_stateful_grid_pass_equals_the_restatement(model, manager):
     rng = np.random.default_rng(23 + int(manager) + 2 * model["centroidalModelType"])
     _, names = abi.builder_desc(model)
     md = abi.motion_desc(model, names, origin) if manager else None
-    emu = E.EmuCenGrid(model, md, B, HORIZON)
+    emu = E.EmuBuilder(model, B, HORIZON, stateful=True, motion=md)
     start = ["stance", "walk", "slow_trot", "run"]
     mgr = [PM(model, filter_origin=origin, state=g) for g in start]
     gs = []
@@ -148,7 +148,7 @@ def test_stateful_grid_pass_equals_the_restatement(model, manager):
         raw = level + rng.normal(0, 0.02, (B, 4))
         x0 = np.array([random_state(model, rng, edges) for _ in range(B)])
         tf = t0 + HORIZON
-        dev = emu.grid(t0, x0, raw, gaits if (c == 0 or not manager) else start, gait_start=[0.5 if g == "stance" else 0.0 for g in start], warm=c > 0)
+        dev = emu.build(t0, x0, raw, gaits if (c == 0 or not manager) else start, gait_start=[0.5 if g == "stance" else 0.0 for g in start], warm=c > 0)
         assert dev["pad_max"] == 0.0, c
         for b in range(B):
             bv = dev["bv"][b]   # bldCenBaseVelocity of x0 (tests/test_emu_cen_builder.py checks it against the oracle)

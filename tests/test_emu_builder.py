@@ -3,7 +3,7 @@ restatement of SolverBase::preRun (references.py): the same checks as tests/test
 import numpy as np
 import pytest
 
-import emu_lib
+import bld_emu_lib
 from wb_humanoid_mpc_b200 import model_loader, references
 from wb_humanoid_mpc_b200.solver import stack_instances
 
@@ -46,7 +46,7 @@ def test_cold_start_arrays_match_the_host_builder(model, gait, start, horizon, t
     rng = np.random.default_rng(abs(int(start * 100)) + len(gait))
     B = 3
     x0s, cmds = make_inputs(model, rng, B)
-    dev = emu_lib.build_instances(model, t0, horizon, x0s, [gait] * B, [start] * B, cmds)
+    dev = bld_emu_lib.build_instances(model, t0, horizon, x0s, [gait] * B, [start] * B, cmds)
     assert not isinstance(dev, int), dev
     host = [references.build_instance(model, x0s[b], t0=t0, horizon=horizon, gait=gait, gait_start=(None if gait == "stance" else start), cmd=list(cmds[b]))
             for b in range(B)]
@@ -58,13 +58,13 @@ def test_warm_start_matches_the_host_shift(model):
     rng = np.random.default_rng(3)
     B, horizon = 2, 1.1
     x0s, cmds = make_inputs(model, rng, B)
-    first = emu_lib.build_instances(model, 0.0, horizon, x0s, ["walk"] * B, [0.0] * B, cmds)
+    first = bld_emu_lib.build_instances(model, 0.0, horizon, x0s, ["walk"] * B, [0.0] * B, cmds)
     n = first["t_nodes"].shape[1]
     xs, us = rng.normal(size=(B, n, 58)), rng.normal(size=(B, n - 1, 35))   # a made-up previous solution on the first grid
     for t1 in (0.1, 0.35, 0.62):
         prevs = [references.to_primal_solution(first["t_nodes"][b], first["node_event"][b], xs[b], us[b]) for b in range(B)]
         x1 = np.array([references.linear_interpolate(t1, p["t"], p["x"]) for p in prevs])
-        dev = emu_lib.build_instances(model, t1, horizon, x1, ["walk"] * B, [0.0] * B, cmds,
+        dev = bld_emu_lib.build_instances(model, t1, horizon, x1, ["walk"] * B, [0.0] * B, cmds,
                                       previous=dict(t=first["t_nodes"], event=first["node_event"], x=xs, u=us))
         host = [references.build_instance(model, x1[b], t0=t1, horizon=horizon, gait="walk", gait_start=0.0, cmd=list(cmds[b]), previous=prevs[b]) for b in range(B)]
         assert dev["t_nodes"].shape[1] == len(host[0]["t_nodes"])
@@ -74,4 +74,4 @@ def test_warm_start_matches_the_host_shift(model):
 def test_mixed_node_counts_are_detected(model):
     rng = np.random.default_rng(1)
     x0s, cmds = make_inputs(model, rng, 2)
-    assert emu_lib.build_instances(model, 0.0, 3.5, x0s, ["walk", "trot"], [0.0, 0.0], cmds) == -2
+    assert bld_emu_lib.build_instances(model, 0.0, 3.5, x0s, ["walk", "trot"], [0.0, 0.0], cmds) == -2

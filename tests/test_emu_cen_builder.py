@@ -6,7 +6,7 @@ the oracle's flow map (full centroidal dynamics) and the closed form of the sing
 import numpy as np
 import pytest
 
-import cen_builder_emu_lib as cbe
+import bld_emu_lib as cbe
 import oracle_lib as orc
 from wb_humanoid_mpc_b200 import centroidal, model_loader, references
 from wb_humanoid_mpc_b200.solver import stack_instances

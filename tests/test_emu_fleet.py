@@ -1,11 +1,10 @@
-"""The fleet's device functions on the CPU harness (tests/emu/fleet_emu.cu): the stable partition by node count (wb_fleet.cuh) against numpy, and
+"""The fleet's device functions on the CPU harness (tests/emu/bld_emu.cu): the stable partition by node count (wb_fleet.cuh) against numpy, and
 the builder's warm start from previous solutions of different lengths per instance (wb_builder.cuh, prevLen + slot map) against the host
 restatement of SolverBase::preRun (references.py)."""
 import numpy as np
 import pytest
 
-import emu_lib
-import fleet_emu_lib
+import bld_emu_lib
 from test_emu_builder import compare, make_inputs
 from wb_humanoid_mpc_b200 import model_loader, references
 
@@ -21,7 +20,7 @@ def test_partition_is_numpys_stable_sort(B, values, threads):
     rng = np.random.default_rng(B + threads)
     nodes = rng.choice(values, B) if values is not None else rng.permutation(np.arange(10, 10 + B))   # None: all counts distinct
     n_bins = int(nodes.max()) + 5
-    slot, groups = fleet_emu_lib.partition(nodes, n_bins, threads)
+    slot, groups = bld_emu_lib.partition(nodes, n_bins, threads)
     assert np.array_equal(slot, np.argsort(nodes, kind="stable"))
     counts = np.bincount(nodes, minlength=n_bins)
     assert [g[0] for g in groups] == np.flatnonzero(counts).tolist()
@@ -50,7 +49,7 @@ def test_warm_build_with_per_instance_previous_lengths(model):
     for t1 in (0.05, 0.3):
         tp = [references.to_primal_solution(p["t"], p["event"], p["x"], p["u"]) for p in prevs]
         x1 = np.array([references.linear_interpolate(t1, p["t"], p["x"]) for p in tp])
-        n, dev = fleet_emu_lib.warm_build(model, t1, horizon, x1, gaits, starts, cmds, prevs)
+        n, dev = bld_emu_lib.warm_build(model, t1, horizon, x1, gaits, starts, cmds, prevs)
         for b in range(B):
             host = references.build_instance(model, x1[b], t0=t1, horizon=horizon, gait=gaits[b], gait_start=(None if gaits[b] == "stance" else starts[b]),
                                              cmd=list(cmds[b]), previous=tp[b])
@@ -80,7 +79,7 @@ def test_stateful_warm_build_with_per_instance_previous_lengths(model):
         schedules.append(gs)
     assert len({len(p["t"]) for p in prevs}) > 1
     x1 = np.array([references.linear_interpolate(t1, p["t"], p["x"]) for p in tp])
-    n, dev = fleet_emu_lib.warm_build(model, t1, horizon, x1, gaits, starts, cmds, prevs, stateful=True, t_prev=0.0)
+    n, dev = bld_emu_lib.warm_build(model, t1, horizon, x1, gaits, starts, cmds, prevs, stateful=True, t_prev=0.0)
     for b in range(B):
         host = references.build_instance(model, x1[b], t0=t1, horizon=horizon, cmd=list(cmds[b]), previous=tp[b], gait_schedule=schedules[b])
         assert n[b] == len(host["t_nodes"])
@@ -88,19 +87,19 @@ def test_stateful_warm_build_with_per_instance_previous_lengths(model):
 
 
 def test_uniform_path_is_unchanged(model):
-    """null prevLen and slot map: bitwise the builder of a plain handle (tests/emu/builder_emu.inc)"""
+    """null prevLen and slot map: bitwise the builder of a plain handle"""
     rng = np.random.default_rng(3)
     B, horizon = 3, 1.1
     x0s, cmds = make_inputs(model, rng, B)
     prevs = previous_solutions(model, rng, ["walk"] * B, [0.0] * B, x0s, cmds, horizon)
-    n, dev = fleet_emu_lib.warm_build(model, 0.2, horizon, x0s, ["walk"] * B, [0.0] * B, cmds, prevs, per_instance=False)
-    ref = emu_lib.build_instances(model, 0.2, horizon, x0s, ["walk"] * B, [0.0] * B, cmds,
+    n, dev = bld_emu_lib.warm_build(model, 0.2, horizon, x0s, ["walk"] * B, [0.0] * B, cmds, prevs, per_instance=False)
+    ref = bld_emu_lib.build_instances(model, 0.2, horizon, x0s, ["walk"] * B, [0.0] * B, cmds,
                                   previous=dict(t=[p["t"] for p in prevs], event=[p["event"] for p in prevs], x=[p["x"] for p in prevs], u=[p["u"] for p in prevs]))
     for b in range(B):
         for k in dev[b]:
             assert np.array_equal(dev[b][k], ref[k][b]), k
     # and the per-instance path with equal lengths gives the same bits
-    n2, dev2 = fleet_emu_lib.warm_build(model, 0.2, horizon, x0s, ["walk"] * B, [0.0] * B, cmds, prevs)
+    n2, dev2 = bld_emu_lib.warm_build(model, 0.2, horizon, x0s, ["walk"] * B, [0.0] * B, cmds, prevs)
     assert np.array_equal(n, n2)
     for b in range(B):
         for k in dev[b]:

@@ -1,4 +1,4 @@
-"""The device builder's stateful gait schedule and trajectorySpread functions (wb_builder.cuh) on the CPU harness (tests/emu/gait_emu.cu):
+"""The device builder's stateful gait schedule and trajectorySpread functions (wb_builder.cuh) on the CPU harness (tests/emu/bld_emu.cu):
 the spreading strategy and its application against the oracle (oracle/trajectory_spreading.hpp) on the reference's 17 recipes and on random
 schedule changes, the inputs against the Python restatement in toPrimalSolution form, and the schedule / updater functions against both host
 restatements over 300 cycles of random gait commands."""
@@ -7,7 +7,7 @@ import bisect
 import numpy as np
 import pytest
 
-import gait_emu_lib as emu
+import bld_emu_lib as emu
 import oracle_lib as orc
 from test_oracle_spreading import CASES, rollout
 from wb_humanoid_mpc_b200 import abi, host_lib, model_loader, references as R

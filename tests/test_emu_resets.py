@@ -1,11 +1,11 @@
-"""Per-instance resets of the device builder on the CPU harness (tests/emu/reset_emu.cu): the automatic predicate over synthetic rows and
+"""Per-instance resets of the device builder on the CPU harness (tests/emu/bld_emu.cu): the automatic predicate over synthetic rows and
 statuses, the episode books and row replacement of builder_reset_kernel, and the warm grid pass with some instances flagged for a reset --
 flagged instances equal a cold pass at the reset time (and the host restatement), the others equal the same warm pass without flags, bit for
 bit."""
 import numpy as np
 import pytest
 
-import reset_emu_lib as E
+import bld_emu_lib as E
 from wb_humanoid_mpc_b200 import abi, model_loader, references as R
 
 NX, CNX = 58, 35
@@ -136,25 +136,27 @@ def test_flagged_instances_restart_cold_and_the_others_are_untouched(model, mana
     B = 8
     names = abi.builder_desc(model)[1]
     md = abi.motion_desc(model, names, 0.0) if manager else None
-    a, b = E.EmuGrid(model, B, HORIZON, md), E.EmuGrid(model, B, HORIZON, md)
+    a = E.EmuBuilder(model, B, HORIZON, stateful=True, motion=md, reset=dict(on=False))   # (requested resets only)
+    b = E.EmuBuilder(model, B, HORIZON, stateful=True, motion=md)
     x0, cmd = _inputs(model, B, rng)
     gaits = ["walk" if i % 2 else "stance" for i in range(B)]
     starts = rng.uniform(0.0, 0.5, B)
     for g in (a, b):
-        g.grid(0.0, x0, cmd, gaits, starts, warm=False)
+        g.build(0.0, x0, cmd, gaits, starts, warm=False)
     for c in range(1, 12):
         for g in (a, b):
-            g.grid(c * DT, x0, cmd, gaits, starts)
+            g.build(c * DT, x0, cmd, gaits, starts)
     t0 = 12 * DT
     flag = np.isin(np.arange(B), [0, 3, 6]).astype(np.uint8)
     rs_gaits = ["walk" if i % 3 else "trot" for i in range(B)]
     rs_off = rng.uniform(-0.4, 0.5, B)
     rs_x0, _ = _inputs(model, B, rng)
     xa = np.where(flag[:, None] == 1, rs_x0, x0)   # builder_reset_kernel has replaced the flagged rows
-    oa = a.grid(t0, xa, cmd, gaits, starts, rst=flag, rs_gaits=rs_gaits, rs_offset=rs_off)
-    ob = b.grid(t0, x0, cmd, gaits, starts)
-    fresh = E.EmuGrid(model, B, HORIZON, abi.motion_desc(model, names, t0) if manager else None)   # a cold pass with every clock at t0
-    oc = fresh.grid(t0, rs_x0, cmd, rs_gaits, t0 + rs_off, warm=False)
+    a.set_reset_states(rs_x0, rs_gaits, rs_off)
+    oa = a.build(t0, x0, cmd, gaits, starts, requests=flag)
+    ob = b.build(t0, x0, cmd, gaits, starts)
+    fresh = E.EmuBuilder(model, B, HORIZON, stateful=True, motion=abi.motion_desc(model, names, t0) if manager else None)   # a cold pass with every clock at t0
+    oc = fresh.build(t0, rs_x0, cmd, rs_gaits, t0 + rs_off, warm=False)
     for i in range(B):
         src = oc if flag[i] else ob
         assert oa["schedules"][i] == src["schedules"][i] and oa["grids"][i] == src["grids"][i], i
@@ -177,7 +179,7 @@ def test_flagged_instances_restart_cold_and_the_others_are_untouched(model, mana
                     assert np.array_equal(oa[k][i], ob[k][i]), k
                 assert oa["origin"][i] == 0.0
     # one pass later the reset instances run warm again from their new episode, with the filter counting from the reset
-    oa2 = a.grid(t0 + DT, xa, cmd, gaits, starts)
+    oa2 = a.build(t0 + DT, xa, cmd, gaits, starts)
     if manager:
         d = DT
         alpha = d / (d + 1 / (2 * np.pi * 5.0))

@@ -141,7 +141,7 @@ def test_one_step_per_cycle_and_the_delay_of_the_targets(model):
 
 # ---- the device functions on the CPU ------------------------------------------------------------------------------------------------------------
 def test_device_filter_and_transitions_equal_the_restatement(model):
-    import motion_emu_lib as E
+    import bld_emu_lib as E
 
     _, names = abi.builder_desc(model)
     md = abi.motion_desc(model, names, 0.3)
@@ -185,13 +185,13 @@ def template(model, gait):
 def test_stateful_grid_pass_with_the_manager_equals_the_restatement(model):
     """300 cycles of random raw commands (the clamp included) and measured base velocities, instances starting in different states: the
     manager state, the gait schedules and the targets of every pass against the restatement driving GaitSchedule.update_gait"""
-    import motion_emu_lib as E
+    import bld_emu_lib as E
 
     B, cycles, origin = 4, 300, -0.05
     rng = np.random.default_rng(17)
     _, names = abi.builder_desc(model)
     md = abi.motion_desc(model, names, origin)
-    emu = E.EmuGrid(model, md, B, HORIZON)
+    emu = E.EmuBuilder(model, B, HORIZON, stateful=True, motion=md)
     start = ["stance", "walk", "slow_trot", "run"]
     mgr = [PM(model, filter_origin=origin, state=g) for g in start]
     gs = []
@@ -215,7 +215,7 @@ def test_stateful_grid_pass_with_the_manager_equals_the_restatement(model):
             x0[b, :4] += rng.uniform(-0.1, 0.1, 4)
         tf = t0 + HORIZON
         # (the stance template started at 0.5 is GaitSchedule's default schedule)
-        dev = emu.grid(t0, x0, raw, gaits=start, gait_start=[0.5 if g == "stance" else 0.0 for g in start], warm=c > 0)
+        dev = emu.build(t0, x0, raw, gaits=start, gait_start=[0.5 if g == "stance" else 0.0 for g in start], warm=c > 0)
         for b in range(B):
             T = tf - t0   # the window of the device, in its arithmetic
             ms = gs[b].get_mode_schedule(t0 - T, tf + T)

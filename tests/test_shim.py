@@ -10,31 +10,27 @@ import pytest
 from wb_humanoid_mpc_b200 import lib
 
 ROOT = Path(__file__).resolve().parents[1]
-BUILD = ROOT / "tests" / "stubs" / "_build"
 
 
-def build_shim_test():
+@pytest.fixture(scope="module")
+def shim_exe(tmp_path_factory):
+    """tests/stubs/shim_test.cpp built once per module in a temporary directory, so that the suite also runs from a read-only tree"""
     lib.lib()   # make sure libb200sqp.so exists
-    BUILD.mkdir(exist_ok=True)
-    exe = BUILD / "shim_test"
-    srcs = [ROOT / "tests" / "stubs" / "shim_test.cpp", ROOT / "tests" / "stubs" / "ocs2_stub.hpp", ROOT / "include" / "ocs2_sqp" / "B200SqpSolver.h",
-            ROOT / "include" / "b200sqp.h"] + list((ROOT / "wb_humanoid_mpc_b200" / "host").glob("*.hpp"))
-    if not exe.exists() or any(s.stat().st_mtime > exe.stat().st_mtime for s in srcs):
-        pkg = ROOT / "wb_humanoid_mpc_b200"
-        subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", f"-I{ROOT / 'include'}", f"-I{ROOT / 'tests' / 'stubs'}", "-o", str(exe), str(srcs[0]), f"-L{pkg}", "-lb200sqp",
-                        "-pthread", f"-Wl,-rpath,{pkg}"], check=True, cwd=ROOT)
+    exe = tmp_path_factory.mktemp("shim") / "shim_test"
+    pkg = ROOT / "wb_humanoid_mpc_b200"
+    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", f"-I{ROOT / 'include'}", f"-I{ROOT / 'tests' / 'stubs'}", "-o", str(exe), str(ROOT / "tests" / "stubs" / "shim_test.cpp"),
+                    f"-L{pkg}", "-lb200sqp", "-pthread", f"-Wl,-rpath,{pkg}"], check=True, cwd=ROOT)
     return exe
 
 
-def run_shim():
-    exe = build_shim_test()
+def run_shim(exe):
     return subprocess.run([str(exe), str(ROOT / "wb_humanoid_mpc_b200" / "data" / "g1_wb_model.txt")], capture_output=True, text=True, cwd=ROOT, timeout=300)
 
 
-def test_shim_compiles_against_stub_ocs2_and_fails_loudly_without_a_device():
+def test_shim_compiles_against_stub_ocs2_and_fails_loudly_without_a_device(shim_exe):
     import torch
 
-    out = run_shim()
+    out = run_shim(shim_exe)
     if torch.cuda.is_available():
         assert out.returncode == 0, out.stdout + out.stderr
     else:
@@ -42,7 +38,7 @@ def test_shim_compiles_against_stub_ocs2_and_fails_loudly_without_a_device():
 
 
 @pytest.mark.gpu
-def test_shim_two_mpc_cycles_match_the_host_layer():
-    out = run_shim()
+def test_shim_two_mpc_cycles_match_the_host_layer(shim_exe):
+    out = run_shim(shim_exe)
     assert out.returncode == 0, out.stdout + out.stderr
     assert "SHIM_OK" in out.stdout
