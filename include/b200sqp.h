@@ -606,6 +606,48 @@ int b200sqp_fleet_joint_actions_dev(b200sqp_fleet f, double t, const double* rob
 int b200sqp_download_dev(b200sqp_handle h, double* x, double* u, double* K, int32_t* status, void* stream);
 int b200sqp_fleet_download_dev(b200sqp_fleet f, int max_nodes, double* x, double* u, double* K, int32_t* status, int32_t* n_nodes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Per-instance gains: the reference's GainsReceiver (humanoid_centroidal_mpc_ros2 src/gains/GainsReceiver.cpp), a synchronized module whose
+ * preSolverRun writes the newest gains message into the OCP's cost and soft-constraint terms, per instance of the batch on the device.
+ * A gain set belongs to one instance index of the built batch (caller order, also on a fleet) and takes effect at that instance's next solve,
+ * stream-ordered behind the work already enqueued on the handle.  Gains persist across solves, warm and cold builds of the same batch size and
+ * per-instance resets; they are dropped (every instance back to the model's values) when the batch size changes, or for the listed instances
+ * by b200sqp_set_gains(..., gains = NULL).  An inactive term (*_active = 0) contributes exactly zero to value, gradient and Hessian of that
+ * instance (its weights, or its penalty's mu, are zero in the instance's model); its stored values come back when it is turned on again.
+ * Gains change the OCP only: the policy roll-outs, the joint-action controller and the builder read the handle's model.  Not tunable: the
+ * equality constraints (switching one off changes the projection sizes), the ICP and external-torque costs, fric_coeff and foot_gain_*.
+ * When gains were never set, solves launch nothing more and compute exactly what they computed before.
+ * b200sqp_default_gains: the handle's model values, every term active.
+ * b200sqp_set_gains: count records for instances [count] (distinct, in [0, B)); gains = NULL restores the model's values.  Every used weight
+ *   must be finite and >= 0, R_diag entries > 0 (the Riccati recursion factorises R~), mu >= 0, delta > 0, radii >= 0, flags 0 or 1:
+ *   B200SQP_EINVAL otherwise, and nothing is applied.  Synchronous like the other host entry points.
+ * b200sqp_download_gains: every instance's current record gains [B] (each may be NULL) and custom [B] (1: set by b200sqp_set_gains).
+ * b200sqp_set_gains_dev: b200sqp_set_gains with the records in device memory (instances on the host), enqueued on `stream` under the
+ *   ordering rules of the device-pointer I/O section.  The checks run on the device per row: status_dev [count] (may be NULL) gets 0 applied,
+ *   1 an entry is not finite, 2 an entry is out of range; a rejected row leaves its instance unchanged.  The first set_gains call at a batch
+ *   size (either path) allocates the per-instance models and waits for the handle's outstanding work; later calls do neither.
+ * B200SQP_ESTATE before a batch exists (b200sqp_set_batch or a build), and on the handle entry points while a fleet is attached.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct b200sqp_gains {
+  double Q_diag[64], R_diag[48], Qf_diag[64];  /* nx / nu entries used: 58 / 35 whole-body, 35 / 35 centroidal */
+  double foot_cost_w[18];                      /* whole-body: EndEffectorDynamicsWeights (18); centroidal: the feet's EndEffectorKinematicsWeights (12) */
+  double torso_w[12];                          /* centroidal: the task-space link's EndEffectorKinematicsWeights; ignored on whole-body handles */
+  double jlim_mu, jlim_delta;                  /* JointLimitsSoftConstraint */
+  double coll_mu, coll_delta, coll_r_foot, coll_r_knee;  /* FootCollisionConstraint and its sphere radii */
+  double fric_mu, fric_delta;                  /* FrictionForceConeConstraint relaxed barrier */
+  double momxy_mu, momxy_delta;                /* ContactMomentXY relaxed barrier */
+  int32_t final_cost_active, foot_cost_active, torso_cost_active, joint_limits_active,
+          foot_collision_active, friction_cone_active, contact_moment_active;
+} b200sqp_gains;
+int b200sqp_default_gains(b200sqp_handle h, b200sqp_gains* out);
+int b200sqp_set_gains(b200sqp_handle h, int count, const int32_t* instances, const b200sqp_gains* gains /* [count] or NULL */);
+int b200sqp_download_gains(b200sqp_handle h, b200sqp_gains* gains /* [B] */, int32_t* custom /* [B] */);
+int b200sqp_set_gains_dev(b200sqp_handle h, int count, const int32_t* instances, const b200sqp_gains* gains_dev, int32_t* status_dev, void* stream);
+int b200sqp_fleet_set_gains(b200sqp_fleet f, int count, const int32_t* instances, const b200sqp_gains* gains);
+int b200sqp_fleet_download_gains(b200sqp_fleet f, b200sqp_gains* gains, int32_t* custom);
+int b200sqp_fleet_set_gains_dev(b200sqp_fleet f, int count, const int32_t* instances, const b200sqp_gains* gains_dev, int32_t* status_dev,
+                                void* stream);
+
 #ifdef __cplusplus
 }
 #endif

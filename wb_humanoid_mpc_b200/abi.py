@@ -319,3 +319,47 @@ class AutoResetDesc(C.Structure):
         ("max_pitch_deviation", C.c_double),
         ("max_roll_deviation", C.c_double),
     ]
+
+
+class Gains(C.Structure):
+    """b200sqp_gains: the per-instance cost weights and soft-constraint penalties of b200sqp_set_gains"""
+    _fields_ = [
+        ("Q_diag", C.c_double * 64),
+        ("R_diag", C.c_double * 48),
+        ("Qf_diag", C.c_double * 64),
+        ("foot_cost_w", C.c_double * 18),
+        ("torso_w", C.c_double * 12),
+        ("jlim_mu", C.c_double), ("jlim_delta", C.c_double),
+        ("coll_mu", C.c_double), ("coll_delta", C.c_double), ("coll_r_foot", C.c_double), ("coll_r_knee", C.c_double),
+        ("fric_mu", C.c_double), ("fric_delta", C.c_double),
+        ("momxy_mu", C.c_double), ("momxy_delta", C.c_double),
+        ("final_cost_active", C.c_int32), ("foot_cost_active", C.c_int32), ("torso_cost_active", C.c_int32), ("joint_limits_active", C.c_int32),
+        ("foot_collision_active", C.c_int32), ("friction_cone_active", C.c_int32), ("contact_moment_active", C.c_int32),
+    ]
+
+
+GAINS_DTYPE = np.dtype(Gains)          # the C layout as a numpy structured dtype (offsets and padding included)
+GAINS_BYTES = C.sizeof(Gains)
+GAIN_FIELDS = [f[0] for f in Gains._fields_]
+
+
+def pack_gains(gains: dict, count: int | None = None) -> np.ndarray:
+    """{field: array with a leading count axis} -> uint8 [count][GAINS_BYTES] in the b200sqp_gains layout (the rows of b200sqp_set_gains, or of
+    b200sqp_set_gains_dev once copied to the device).  Every field is required; with `count` given, a single record's values are repeated."""
+    missing = [k for k in GAIN_FIELDS if k not in gains]
+    if missing:
+        raise KeyError(f"pack_gains: missing fields {missing}")
+    if count is None:
+        count = int(np.shape(gains["final_cost_active"])[0]) if np.ndim(gains["final_cost_active"]) else 1
+    rec = np.zeros(count, dtype=GAINS_DTYPE)
+    for k in GAIN_FIELDS:
+        rec[k] = gains[k]
+    return rec.view(np.uint8).reshape(count, GAINS_BYTES)
+
+
+def unpack_gains(rec: np.ndarray) -> dict:
+    """uint8 [count][GAINS_BYTES] (or a GAINS_DTYPE array) -> {field: array with a leading count axis}"""
+    rec = np.ascontiguousarray(rec)
+    if rec.dtype != GAINS_DTYPE:
+        rec = rec.reshape(-1, GAINS_BYTES).view(GAINS_DTYPE).reshape(-1)
+    return {k: rec[k].copy() for k in GAIN_FIELDS}

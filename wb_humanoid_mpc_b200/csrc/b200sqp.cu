@@ -29,6 +29,7 @@
 #include "wb_devio.cuh"
 #include "cen_kernels.cuh"
 #include "cen_host.cuh"
+#include "wb_gains.cuh"
 #endif
 
 namespace {

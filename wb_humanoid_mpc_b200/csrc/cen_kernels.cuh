@@ -26,8 +26,9 @@ __global__ void __launch_bounds__(CEN_THREADS) cen_lq_kernel(WbDev d, const CenD
     n.u = d.u + stage * NU;
     n.xnext = d.x + (node + 1) * NX;
   }
-  if (lqTerminalOrEventNode(d, n, k, node, stage, cm->QfdPad, CNX, CNU, smem)) return;
-  const CenOcpModel& m = cm->ocp;
+  const CenDevModel& mb = cm[static_cast<size_t>(b) * d.modelStride];   // the instance's gains (stride 0: the handle's model)
+  if (lqTerminalOrEventNode(d, n, k, node, stage, mb.QfdPad, CNX, CNU, smem)) return;
+  const CenOcpModel& m = mb.ocp;
   CenLqWs s;
   cenLqWsMap(smem, s);
   double* const raw = d.raw + stage * d.rawPer;
@@ -71,12 +72,13 @@ __global__ void __launch_bounds__(32) cen_rollout_kernel(WbDev d, const CenDevMo
   n.x = xa;
   n.u = ua;
   n.xnext = xna;
+  const CenDevModel& mb = cm[static_cast<size_t>(b) * d.modelStride];
   if (k == N || n.event == 1) {
     double c = 0.0;
     for (int i = 0; i < NX; ++i) {
       if (k == N) {
         const double dx = xa[i] - n.xref[i];
-        c += 0.5 * cm->QfdPad[i] * dx * dx;
+        c += 0.5 * mb.QfdPad[i] * dx * dx;
       } else {
         const double df = xa[i] - xna[i];
         c += df * df;
@@ -87,7 +89,7 @@ __global__ void __launch_bounds__(32) cen_rollout_kernel(WbDev d, const CenDevMo
     perfOut[2] = 0.0;
     return;
   }
-  const CenOcpModel& m = cm->ocp;
+  const CenOcpModel& m = mb.ocp;
   CenKin kin;
   cenTorsoReference(m, n.xref, kin, tref);
   CenDirOut o;

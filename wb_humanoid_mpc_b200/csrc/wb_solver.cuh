@@ -67,9 +67,16 @@ enum InstD { I_BASE_MERIT = 0, I_BASE_COST, I_BASE_DYN, I_BASE_EQ, I_ARMIJO, I_D
              I_NEW_DYN, I_NEW_EQ, I_ND = 16 };
 enum InstF { F_CONVERGED = 0, F_LSDONE, F_ITER, F_STATUS, F_CONVCODE, F_RANKDEF, F_NF = 8 };
 
+struct CenDevModel;
+
 struct WbDev {
   int B, N;  // N intervals, N+1 nodes
-  const WbDeviceModel* model;
+  const WbDeviceModel* model;   // the handle's model (roll-outs, joint actions, builder)
+  // the OCP's model of instance b (cost and penalty kernels): instModel[b * modelStride] (whole-body), instCen[b * modelStride] (centroidal);
+  // the handle's model with stride 0 until per-instance gains are set (wb_gains.cuh)
+  const WbDeviceModel* instModel;
+  const CenDevModel* instCen;
+  int modelStride;
   // instance inputs
   double *x0, *x, *u, *t, *swing, *impact, *arm, *xref;
   double *xInit, *uInit;  // uploaded initial guess (restored by b200sqp_reset)
@@ -248,13 +255,14 @@ __global__ void __launch_bounds__(LQA_THREADS, B200SQP_LQA_CTAS) lq_dyn_kernel(W
     n.u = d.u + stage * NU;
     n.xnext = d.x + (node + 1) * NX;
   }
-  if (lqTerminalOrEventNode(d, n, k, node, stage, d.model->Qfd, NX, NU, smem)) return;
+  const WbDeviceModel* const mb = d.instModel + static_cast<size_t>(b) * d.modelStride;
+  if (lqTerminalOrEventNode(d, n, k, node, stage, mb->Qfd, NX, NU, smem)) return;
 #if B200SQP_LQA_GLOBAL_MODEL
-  const WbDeviceModel& m = *d.model;   // read through L1 (8.7 KB, shared by every CTA of the SM): the shared memory buys a fourth node
+  const WbDeviceModel& m = *mb;   // read through L1 (8.7 KB, shared by every CTA of the SM): the shared memory buys a fourth node
 #else
   __shared__ WbDeviceModel msh;  // model constants staged once per CTA: the kinematic phases read them in dependent sequences
   for (int i = threadIdx.x; i < static_cast<int>(sizeof(WbDeviceModel) / 8); i += blockDim.x)
-    reinterpret_cast<double*>(&msh)[i] = reinterpret_cast<const double*>(d.model)[i];
+    reinterpret_cast<double*>(&msh)[i] = reinterpret_cast<const double*>(mb)[i];
   __syncthreads();
   const WbDeviceModel& m = msh;
 #endif
@@ -574,9 +582,7 @@ __device__ __forceinline__ void rolloutNodes(const WbDev& d, const WbDeviceModel
 // sixteenth of the rows (the asynchronous solve enqueues the whole back-tracking ladder, wb_capi.inc).
 __global__ void __launch_bounds__(RO_THREADS, B200SQP_RO_CTAS) rollout_kernel(WbDev d) {
   extern __shared__ double smem[];
-#if B200SQP_RO_GLOBAL_MODEL
-  const WbDeviceModel& msh = *d.model;   // read through L1 (8.7 KB, shared by every CTA of the SM) instead of one copy per CTA
-#else
+#if !B200SQP_RO_GLOBAL_MODEL
   __shared__ WbDeviceModel msh;
 #endif
   __shared__ NodeIn nsh[RO_PACK];
@@ -596,11 +602,15 @@ __global__ void __launch_bounds__(RO_THREADS, B200SQP_RO_CTAS) rollout_kernel(Wb
   __syncthreads();
   const int n = nAct;
   if (n == 0) return;
-#if !B200SQP_RO_GLOBAL_MODEL
-  for (int i = threadIdx.x; i < static_cast<int>(sizeof(WbDeviceModel) / 8); i += blockDim.x)
-    reinterpret_cast<double*>(&msh)[i] = reinterpret_cast<const double*>(d.model)[i];
+  for (int a = 0; a < n; ++a) {   // (the instances of one CTA may carry different gains: the model is looked up per instance)
+    const WbDeviceModel* const mb = d.instModel + static_cast<size_t>(act[a]) * d.modelStride;
+#if B200SQP_RO_GLOBAL_MODEL
+    const WbDeviceModel& msh = *mb;   // read through L1 (8.7 KB, shared by every CTA of the SM) instead of one copy per CTA
+#else
+    for (int i = threadIdx.x; i < static_cast<int>(sizeof(WbDeviceModel) / 8); i += blockDim.x)
+      reinterpret_cast<double*>(&msh)[i] = reinterpret_cast<const double*>(mb)[i];
+    __syncthreads();
 #endif
-  for (int a = 0; a < n; ++a) {
     rolloutNodes(d, msh, nsh, smem, act[a], k0);
     __syncthreads();   // the workspace is reused by the next instance
   }

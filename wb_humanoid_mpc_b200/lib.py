@@ -184,4 +184,11 @@ EXPORTED_SYMBOLS = [
     "b200sqp_fleet_joint_actions_dev",
     "b200sqp_download_dev",
     "b200sqp_fleet_download_dev",
+    "b200sqp_default_gains",
+    "b200sqp_set_gains",
+    "b200sqp_download_gains",
+    "b200sqp_set_gains_dev",
+    "b200sqp_fleet_set_gains",
+    "b200sqp_fleet_download_gains",
+    "b200sqp_fleet_set_gains_dev",
 ]

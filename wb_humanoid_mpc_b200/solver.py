@@ -136,6 +136,32 @@ def _joint_actions_device(fn, h, device, B, nx, nu, nj, t, robot_state, use_poli
     return o
 
 
+def _set_gains(fn, h, indices, gains):
+    idx = np.ascontiguousarray(np.atleast_1d(indices), dtype=np.int32)
+    rec = None if gains is None else abi.pack_gains(gains, idx.size if np.ndim(gains["final_cost_active"]) == 0 else None)
+    if rec is not None and rec.shape[0] != idx.size:
+        raise ValueError(f"set_gains: {rec.shape[0]} gain records for {idx.size} instances")
+    _l.check(fn(h, C.c_int(idx.size), idx.ctypes.data_as(_l.ip), None if rec is None else rec.ctypes.data_as(C.c_void_p)))
+
+
+def _gains(fn, h, B) -> dict:
+    rec, custom = np.zeros((B, abi.GAINS_BYTES), dtype=np.uint8), np.zeros(B, dtype=np.int32)
+    _l.check(fn(h, rec.ctypes.data_as(C.c_void_p), custom.ctypes.data_as(_l.ip)))
+    out = abi.unpack_gains(rec)
+    out["custom"] = custom.astype(bool)
+    return out
+
+
+def _set_gains_device(fn, h, device, indices, gains, stream):
+    import torch
+
+    idx = np.ascontiguousarray(np.atleast_1d(indices), dtype=np.int32)
+    g = check_device_tensor(gains, "gains", device, torch.uint8, (idx.size, abi.GAINS_BYTES))
+    status = torch.empty(idx.size, dtype=torch.int32, device=device)
+    _l.check(fn(h, C.c_int(idx.size), idx.ctypes.data_as(_l.ip), _vp(g), _vp(status), _stream(device, stream)))
+    return status
+
+
 def stack_instances(instances: list[dict]) -> dict:
     """list of per-instance dicts (references.build_instance) -> batched arrays; all instances must share the node count."""
     n = {len(i["t_nodes"]) for i in instances}
@@ -368,6 +394,30 @@ class B200SqpSolver:
         """b200sqp_download_pose_targets: {active [B] (bool), t_start [B], t_reach [B], target_pose [B, 6], error [B, 2] (planar distance and
         |yaw error| of the last build's measured state)}"""
         return _pose_targets(_l.lib().b200sqp_download_pose_targets, self._h, self.batch)
+
+    # -- per-instance gains (the reference's GainsReceiver, per instance on the device) ---------------------------------------------
+    def default_gains(self) -> dict:
+        """b200sqp_default_gains: the model's cost weights and penalties, every term active, as {field of abi.Gains: value}"""
+        g = abi.Gains()
+        _l.check(_l.lib().b200sqp_default_gains(self._h, C.byref(g)))
+        return {k: v[0] for k, v in abi.unpack_gains(np.frombuffer(bytes(g), dtype=np.uint8)).items()}
+
+    def set_gains(self, indices, gains: dict | None):
+        """b200sqp_set_gains: gains {field: array with a leading len(indices) axis} (a default_gains()-shaped dict applies to every listed
+        instance), or None to restore the model's values; takes effect at each instance's next solve"""
+        _set_gains(_l.lib().b200sqp_set_gains, self._h, indices, gains)
+
+    def gains(self) -> dict:
+        """b200sqp_download_gains: {field: [B, ...]} and custom [B] (bool: set by set_gains)"""
+        return _gains(_l.lib().b200sqp_download_gains, self._h, self.batch)
+
+    def set_gains_device(self, indices, gains, stream=None):
+        """b200sqp_set_gains_dev: gains a uint8 CUDA tensor [len(indices), abi.GAINS_BYTES] in the b200sqp_gains layout (abi.pack_gains),
+        checked and applied per row on the device on `stream` (None: the current torch stream); returns the int32 status tensor (0 applied,
+        1 an entry is not finite, 2 out of range)"""
+        import torch
+
+        return _set_gains_device(_l.lib().b200sqp_set_gains_dev, self._h, torch.device("cuda", self.device), indices, gains, stream)
 
     def mode_schedule(self, max_events: int = 192) -> list:
         """the window mode schedule of every instance that the last build_instances used: [(event_times, mode_sequence)] * B"""
@@ -643,6 +693,23 @@ class B200SqpFleet:
     def pose_targets(self) -> dict:
         """B200SqpSolver.pose_targets of the fleet's instances (caller order)"""
         return _pose_targets(_l.lib().b200sqp_fleet_download_pose_targets, self._f, self.batch)
+
+    def default_gains(self) -> dict:
+        return self.solver.default_gains()
+
+    def set_gains(self, indices, gains: dict | None):
+        """B200SqpSolver.set_gains for the fleet's instances (caller order)"""
+        _set_gains(_l.lib().b200sqp_fleet_set_gains, self._f, indices, gains)
+
+    def gains(self) -> dict:
+        """B200SqpSolver.gains of the fleet's instances (caller order)"""
+        return _gains(_l.lib().b200sqp_fleet_download_gains, self._f, self.batch)
+
+    def set_gains_device(self, indices, gains, stream=None):
+        """B200SqpSolver.set_gains_device for the fleet's instances (caller order)"""
+        import torch
+
+        return _set_gains_device(_l.lib().b200sqp_fleet_set_gains_dev, self._f, torch.device("cuda", self.solver.device), indices, gains, stream)
 
     def mode_schedule(self, max_events: int = 192) -> list:
         B = self.batch
