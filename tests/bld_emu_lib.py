@@ -25,12 +25,17 @@ def lib():
         L = C.CDLL(str(build("bld_emu.cu", "libbldemu.so")))
         L.emu_bld_create.restype = C.c_void_p
         L.emu_gait_create.restype = C.c_void_p
+        L.emu_batch_member.restype = C.c_char_p
         _lib = L
     return _lib
 
 
 def _u8(a):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8))
+
+
+def _i64(a):
+    return a.ctypes.data_as(C.POINTER(C.c_longlong))
 
 
 def pad(a):
@@ -279,6 +284,45 @@ def partition(nodes, n_bins, threads=1024):
     slot, gtab = np.zeros(len(nodes), dtype=np.int32), np.zeros(1 + 3 * n_bins, dtype=np.int32)
     lib().emu_fleet_partition(_pi(nodes), C.c_int(len(nodes)), C.c_int(n_bins), C.c_int(threads), _pi(slot), _pi(gtab))
     return slot, [tuple(gtab[1 + 3 * g: 4 + 3 * g]) for g in range(gtab[0])]
+
+
+# ---- the batch layout (wb_batch.cuh) ---------------------------------------------------------------------------------------------------------------
+ROW_KINDS = ("instance", "node", "stage", "handle")
+MAX_ENTRIES = 64
+
+
+def _layout_args(cen, value_function, feedback, raw, max_iter, raw_per):
+    return (C.c_int(int(cen)), C.c_int(int(value_function)), C.c_int(int(feedback)), C.c_int(int(raw)), C.c_int(max_iter), C.c_longlong(raw_per))
+
+
+def batch_layout(cen, value_function, feedback, raw, max_iter, raw_per):
+    """forEachBatchArray of a handle with these settings (max_iter, raw_per: the widths of log and raw) -> [(member name, row kind, width,
+    zero fill)] in allocation order"""
+    L = lib()
+    member, kind, zero = (np.zeros(MAX_ENTRIES, np.int32) for _ in range(3))
+    width = np.zeros(MAX_ENTRIES, np.int64)
+    n = L.emu_batch_layout(*_layout_args(cen, value_function, feedback, raw, max_iter, raw_per), _pi(member), _pi(kind), _i64(width), _pi(zero))
+    assert (member[:n] >= 0).all(), "an entry of the table is no array member of WbDev"
+    return [(L.emu_batch_member(int(m)).decode(), ROW_KINDS[k], int(w), bool(z)) for m, k, w, z in zip(member[:n], kind[:n], width[:n], zero[:n])]
+
+
+def group_views(cen, value_function, feedback, raw, max_iter, raw_per, B, cap, groups):
+    """the table's allocation of B instances at cap nodes, then groupView of every (n, first, count) of groups -> (bytes [E] allocated per
+    entry, offsets [G, E] of each view's pointer into the entry's allocation in bytes, -1 for null), entries in allocation order"""
+    gtab = np.array([len(groups), *(v for g in groups for v in g)], np.int32)
+    bytes_, off = np.zeros(MAX_ENTRIES, np.int64), np.zeros(len(groups) * MAX_ENTRIES, np.int64)
+    n = lib().emu_group_views(*_layout_args(cen, value_function, feedback, raw, max_iter, raw_per), C.c_int(B), C.c_int(cap), _pi(gtab), _i64(bytes_),
+                              _i64(off))
+    return bytes_[:n], off[: len(groups) * n].reshape(len(groups), n)
+
+
+def fleet_slots(groups, B, cap):
+    """fleetSlot of every slot (groups None: a plain handle) -> dict(n, first, count, node, stage) of [B] arrays"""
+    gtab = None if groups is None else np.array([len(groups), *(v for g in groups for v in g)], np.int32)
+    out = dict(n=np.zeros(B, np.int32), first=np.zeros(B, np.int32), count=np.zeros(B, np.int32), node=np.zeros(B, np.int64), stage=np.zeros(B, np.int64))
+    lib().emu_fleet_slots(None if gtab is None else _pi(gtab), C.c_int(B), C.c_int(cap), _pi(out["n"]), _pi(out["first"]), _pi(out["count"]),
+                          _i64(out["node"]), _i64(out["stage"]))
+    return out
 
 
 def base_velocity(model, x):

@@ -1,10 +1,13 @@
-// DEVELOPMENT HARNESS (tests only, never linked into libb200sqp.so): the device builder (wb_builder.cuh) and the fleet's partition (wb_fleet.cuh)
-// executed on the CPU.  One context holds B instances' builder state the way the handle's batch allocation does, and emu_bld_build runs the
-// work items in the order b200sqp_build_instances launches its kernels, every loop in reverse so that an order dependence shows as a mismatch.
+// DEVELOPMENT HARNESS (tests only, never linked into libb200sqp.so): the device builder (wb_builder.cuh), the fleet's partition and slot helper
+// (wb_fleet.cuh) and the batch layout (wb_batch.cuh) executed on the CPU.  One context holds B instances' builder state the way the handle's batch
+// allocation does, and emu_bld_build runs the work items in the order b200sqp_build_instances launches its kernels, every loop in reverse so that
+// an order dependence shows as a mismatch.
 // Built into tests/emu/libbldemu.so by tests/bld_emu_lib.py.  The product has no CPU path.
 #include <cmath>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "../../wb_humanoid_mpc_b200/csrc/cen_host.cuh"
@@ -233,39 +236,26 @@ int emu_bld_build(void* cp, int warm, double t0, double horizon, const double* x
     if (c.scratch[i].overflow) return -1;
     c.nNodes[i] = c.scratch[i].nNodes;
   }
+  d.x = c.x.data();
+  d.u = c.u.data();
+  d.t = c.t.data();
+  d.event = c.event.data();
+  d.contact = c.contact.data();
+  d.swing = c.swing.data();
+  d.impact = c.impact.data();
+  d.arm = c.arm.data();
+  d.xref = c.xref.data();
   if (nodes == 1) {
     const int n = c.nNodes[0];
     for (int i = 0; i < B; ++i)
       if (c.nNodes[i] != n) return -2;
     d.N = n - 1;
-    d.x = c.x.data();
-    d.u = c.u.data();
-    d.t = c.t.data();
-    d.event = c.event.data();
-    d.contact = c.contact.data();
-    d.swing = c.swing.data();
-    d.impact = c.impact.data();
-    d.arm = c.arm.data();
-    d.xref = c.xref.data();
     for (int i = B - 1; i >= 0; --i)
       for (int k = n - 1; k >= 0; --k)
         for (int tid = 63; tid >= 0; --tid) bldNode(d, b, k, i, tid, 64);
   } else if (nodes == 2) {
     for (int i = B - 1; i >= 0; --i) {   // instance i as position 0 of a fleet group of size 1 at slot i
-      const size_t node = static_cast<size_t>(i) * cap, stage = static_cast<size_t>(i) * (cap - 1);
-      WbDev v{};
-      v.B = 1;
-      v.N = c.nNodes[i] - 1;
-      v.x0 = c.x0.data() + static_cast<size_t>(i) * NX;
-      v.x = c.x.data() + node * NX;
-      v.u = c.u.data() + stage * NU;
-      v.t = c.t.data() + node;
-      v.event = c.event.data() + node;
-      v.contact = c.contact.data() + node * 2;
-      v.swing = c.swing.data() + node * 6;
-      v.impact = c.impact.data() + node * 2;
-      v.arm = c.arm.data() + node;
-      v.xref = c.xref.data() + node * NX;
+      const WbDev v = groupView(d, cap, c.nNodes[i], i, 1, nullptr);
       BldDev bi = b;
       bi.slot = &i;
       for (int k = v.N; k >= 0; --k)
@@ -491,6 +481,95 @@ void emu_fleet_partition(const int* nodes, int B, int nBins, int nt, int* slotIn
   for (int tile = 0; tile < B; tile += nt) {
     for (int t = nt - 1; t >= 0; --t) fleetPlace(key.data(), B, cnt.data(), slotInst, tile, t);
     for (int t = 0; t < nt; ++t) fleetAdvance(key.data(), B, cnt.data(), tile, t);
+  }
+}
+
+// ---- the batch layout (wb_batch.cuh) ---------------------------------------------------------------------------------------------------------------
+namespace {
+#define WB_M(f) {#f, offsetof(WbDev, f)}
+#define WB_Q(f) {"qp." #f, offsetof(WbDev, qp) + offsetof(QpDeviceView, f)}
+// the array members of WbDev by name
+const struct {
+  const char* name;
+  size_t off;
+} kMembers[] = {WB_M(x0),   WB_M(x),       WB_M(u),        WB_M(t),     WB_M(swing), WB_M(impact),  WB_M(arm),    WB_M(xref),   WB_M(xInit),
+                WB_M(uInit), WB_M(event),  WB_M(contact),  WB_Q(A),     WB_Q(Bm),    WB_Q(b),       WB_Q(Q),      WB_Q(S),      WB_Q(R),
+                WB_Q(q),     WB_Q(r),      WB_Q(dx0),      WB_Q(nu),    WB_Q(K),     WB_Q(kff),     WB_Q(P),      WB_Q(p),      WB_Q(dx),
+                WB_Q(du),    WB_Q(status), WB_M(Pu),       WB_M(Px),    WB_M(u0p),   WB_M(du),      WB_M(Kre),    WB_M(perfNode), WB_M(lsNode),
+                WB_M(inst),  WB_M(flags),  WB_M(pending),  WB_M(mid),   WB_M(luRec), WB_M(luPerm),  WB_M(gstats), WB_M(raw),    WB_M(log)};
+#undef WB_M
+#undef WB_Q
+
+// a handle's device state as set_batch walks the table: the settings and the widths the table reads
+WbDev layoutBase(int valueFunction, int feedback, int maxIter, long long rawPer) {
+  WbDev d{};
+  d.st.create_value_function = valueFunction;
+  d.st.use_feedback_policy = feedback;
+  d.maxIter = maxIter;
+  d.rawPer = rawPer;
+  d.qp.nx = NX;
+  d.qp.numax = NUT_MAX;
+  return d;
+}
+}  // namespace
+
+const char* emu_batch_member(int i) { return kMembers[i].name; }
+
+// forEachBatchArray of a handle with these settings: for entry e, member[e] (emu_batch_member; -1 for a field that is no array member), its
+// row kind kind[e] (0 instance, 1 node, 2 stage, 3 handle), its elements per row width[e] and its zero fill zero[e].  Returns the entries.
+int emu_batch_layout(int cen, int value_function, int feedback, int raw, int max_iter, long long raw_per, int* member, int* kind, long long* width,
+                     int* zero) {
+  WbDev d = layoutBase(value_function, feedback, max_iter, raw_per);
+  int e = 0;
+  forEachBatchArray(d, cen, raw, [&](auto*& p, RowKind k, size_t w, bool z) {
+    const size_t off = reinterpret_cast<const char*>(&p) - reinterpret_cast<const char*>(&d);
+    member[e] = -1;
+    for (size_t i = 0; i < sizeof(kMembers) / sizeof(kMembers[0]); ++i)
+      if (kMembers[i].off == off) member[e] = static_cast<int>(i);
+    kind[e] = k;
+    width[e] = static_cast<long long>(w);
+    zero[e] = z;
+    ++e;
+  });
+  return e;
+}
+
+// The allocation of B instances at cap nodes per instance by walking the table (as set_batch does), then groupView of every group of gtab
+// {G, (n, first, count) * G} with a null line-search counter: bytes[e] allocated for entry e, and off[g * E + e] the byte offset of group g's
+// pointer into that allocation (-1: null).  Returns the number of entries E.
+int emu_group_views(int cen, int value_function, int feedback, int raw, int max_iter, long long raw_per, int B, int cap, const int* gtab,
+                    long long* bytes, long long* off) {
+  WbDev d = layoutBase(value_function, feedback, max_iter, raw_per);
+  std::vector<const char*> base;
+  forEachBatchArray(d, cen, raw, [&](auto*& p, RowKind k, size_t w, bool) {
+    const size_t n = batchRows(k, B, cap) * w * sizeof(*p);
+    p = static_cast<std::remove_reference_t<decltype(p)>>(std::malloc(n));
+    bytes[base.size()] = static_cast<long long>(n);
+    base.push_back(reinterpret_cast<const char*>(p));
+  });
+  const int E = static_cast<int>(base.size());
+  for (int g = 0; g < gtab[0]; ++g) {
+    WbDev v = groupView(d, cap, gtab[1 + 3 * g], gtab[2 + 3 * g], gtab[3 + 3 * g], nullptr);
+    int e = 0;
+    forEachBatchArray(v, cen, raw, [&](auto*& p, RowKind, size_t, bool) {
+      off[g * E + e] = p ? reinterpret_cast<const char*>(p) - base[e] : -1;
+      ++e;
+    });
+  }
+  for (const char* p : base) std::free(const_cast<char*>(p));
+  return E;
+}
+
+// fleetSlot of every slot s < B of a batch at cap nodes per instance (gtab NULL: a plain handle): its group's n, first, count [B] and its first
+// node and stage rows [B]
+void emu_fleet_slots(const int* gtab, int B, int cap, int* n, int* first, int* count, long long* node, long long* stage) {
+  for (int s = 0; s < B; ++s) {
+    const FleetSlot r = fleetSlot(gtab, B, cap, s);
+    n[s] = r.n;
+    first[s] = r.first;
+    count[s] = r.count;
+    node[s] = static_cast<long long>(r.node);
+    stage[s] = static_cast<long long>(r.stage);
   }
 }
 

@@ -169,12 +169,9 @@ class MemOwner {
 }  // namespace b200sqp
 
 struct b200sqp_qp_t {
-  int device = 0, B = 0, N = 0, nx = 0, numax = 0;
-  double *A = nullptr, *Bm = nullptr, *b = nullptr, *Q = nullptr, *S = nullptr, *R = nullptr, *q = nullptr, *r = nullptr, *dx0 = nullptr;
-  int* nu = nullptr;
+  int device = 0;
+  b200sqp::QpDeviceView v{};   // the arrays and sizes; a solve sets nu, keepP and reg on its copy
   bool hasNu = false;
-  double *K = nullptr, *kff = nullptr, *P = nullptr, *p = nullptr, *dx = nullptr, *du = nullptr;
-  int* status = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   bool uploaded = false, solved = false, keptP = false;
   b200sqp::MemOwner mem;
@@ -194,29 +191,13 @@ int b200sqp_qp_create(int device, int batch, int N, int nx, int nu_max, b200sqp_
   b200sqp_qp_t* qp = new (std::nothrow) b200sqp_qp_t;
   if (!qp) return fail(B200SQP_ENOMEM, "host allocation failed");
   qp->device = device;
-  qp->B = batch;
-  qp->N = N;
-  qp->nx = nx;
-  qp->numax = nu_max;
-  const size_t bn = static_cast<size_t>(batch) * N, bn1 = static_cast<size_t>(batch) * (N + 1);
+  b200sqp::QpDeviceView& v = qp->v;
+  v.B = batch;
+  v.N = N;
+  v.nx = nx;
+  v.numax = nu_max;
   b200sqp::MemOwner& m = qp->mem;
-  m.device(qp->A, bn * nx * nx);
-  m.device(qp->Bm, bn * nx * nu_max);
-  m.device(qp->b, bn * nx);
-  m.device(qp->Q, bn1 * nx * nx);
-  m.device(qp->S, bn * nu_max * nx);
-  m.device(qp->R, bn * nu_max * nu_max);
-  m.device(qp->q, bn1 * nx);
-  m.device(qp->r, bn * nu_max);
-  m.device(qp->dx0, static_cast<size_t>(batch) * nx);
-  m.device(qp->nu, bn);
-  m.device(qp->K, bn * nu_max * nx);
-  m.device(qp->kff, bn * nu_max);
-  m.device(qp->P, bn1 * nx * nx);
-  m.device(qp->p, bn1 * nx);
-  m.device(qp->dx, bn1 * nx);
-  m.device(qp->du, bn * nu_max);
-  m.device(qp->status, batch);
+  b200sqp::forEachQpArray(v, true, [&](auto*& a, b200sqp::RowKind k, int w) { m.device(a, b200sqp::batchRows(k, batch, N + 1) * w); });
   cudaError_t e = m.error();
   if (e == cudaSuccess) e = cudaEventCreate(&qp->ev0);
   if (e == cudaSuccess) e = cudaEventCreate(&qp->ev1);
@@ -241,23 +222,25 @@ int b200sqp_qp_upload(b200sqp_qp qp, const double* A, const double* B, const dou
                       const double* R, const double* q, const double* r, const int32_t* nu, const double* dx0) {
   if (!qp || !A || !B || !b || !Q || !S || !R || !q || !r || !dx0) return fail(B200SQP_EINVAL, "qp_upload: null argument");
   CUDA_TRY(cudaSetDevice(qp->device));
-  const size_t bn = static_cast<size_t>(qp->B) * qp->N, bn1 = static_cast<size_t>(qp->B) * (qp->N + 1);
-  const int nx = qp->nx, nm = qp->numax;
-  auto up = [&](double* d, const double* h, size_t n) { return cudaMemcpy(d, h, n * sizeof(double), cudaMemcpyHostToDevice); };
-  CUDA_TRY(up(qp->A, A, bn * nx * nx));
-  CUDA_TRY(up(qp->Bm, B, bn * nx * nm));
-  CUDA_TRY(up(qp->b, b, bn * nx));
-  CUDA_TRY(up(qp->Q, Q, bn1 * nx * nx));
-  CUDA_TRY(up(qp->S, S, bn * nm * nx));
-  CUDA_TRY(up(qp->R, R, bn * nm * nm));
-  CUDA_TRY(up(qp->q, q, bn1 * nx));
-  CUDA_TRY(up(qp->r, r, bn * nm));
-  CUDA_TRY(up(qp->dx0, dx0, static_cast<size_t>(qp->B) * nx));
+  const b200sqp::QpDeviceView& v = qp->v;
+  const size_t bn = static_cast<size_t>(v.B) * v.N, bn1 = static_cast<size_t>(v.B) * (v.N + 1);
+  const int nx = v.nx, nm = v.numax;
+  // (the inputs are const in the view the kernels read)
+  auto up = [&](const void* d, const void* h, size_t bytes) { return cudaMemcpy(const_cast<void*>(d), h, bytes, cudaMemcpyHostToDevice); };
+  CUDA_TRY(up(v.A, A, bn * nx * nx * sizeof(double)));
+  CUDA_TRY(up(v.Bm, B, bn * nx * nm * sizeof(double)));
+  CUDA_TRY(up(v.b, b, bn * nx * sizeof(double)));
+  CUDA_TRY(up(v.Q, Q, bn1 * nx * nx * sizeof(double)));
+  CUDA_TRY(up(v.S, S, bn * nm * nx * sizeof(double)));
+  CUDA_TRY(up(v.R, R, bn * nm * nm * sizeof(double)));
+  CUDA_TRY(up(v.q, q, bn1 * nx * sizeof(double)));
+  CUDA_TRY(up(v.r, r, bn * nm * sizeof(double)));
+  CUDA_TRY(up(v.dx0, dx0, static_cast<size_t>(v.B) * nx * sizeof(double)));
   qp->hasNu = nu != nullptr;
   if (nu) {
     for (size_t i = 0; i < bn; ++i)
       if (nu[i] < 0 || nu[i] > nm) return fail(B200SQP_EINVAL, "qp_upload: nu[%zu]=%d outside [0,%d]", i, nu[i], nm);
-    CUDA_TRY(cudaMemcpy(qp->nu, nu, bn * sizeof(int), cudaMemcpyHostToDevice));
+    CUDA_TRY(up(v.nu, nu, bn * sizeof(int)));
   }
   qp->uploaded = true;
   qp->solved = false;
@@ -269,34 +252,14 @@ int b200sqp_qp_solve(b200sqp_qp qp, double reg_prim, int keep_P, void* stream) {
   if (!qp->uploaded) return fail(B200SQP_ESTATE, "qp_solve: no problem uploaded");
   CUDA_TRY(cudaSetDevice(qp->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t bn = static_cast<size_t>(qp->B) * qp->N;
-  b200sqp::QpDeviceView v{};
-  v.B = qp->B;
-  v.N = qp->N;
-  v.nx = qp->nx;
-  v.numax = qp->numax;
-  v.A = qp->A;
-  v.Bm = qp->Bm;
-  v.b = qp->b;
-  v.Q = qp->Q;
-  v.S = qp->S;
-  v.R = qp->R;
-  v.q = qp->q;
-  v.r = qp->r;
-  v.dx0 = qp->dx0;
-  v.nu = qp->hasNu ? qp->nu : nullptr;
-  v.K = qp->K;
-  v.kff = qp->kff;
-  v.P = qp->P;
-  v.p = qp->p;
-  v.dx = qp->dx;
-  v.du = qp->du;
-  v.status = qp->status;
+  const size_t bn = static_cast<size_t>(qp->v.B) * qp->v.N;
+  b200sqp::QpDeviceView v = qp->v;
+  if (!qp->hasNu) v.nu = nullptr;
   v.keepP = keep_P;
   v.reg = reg_prim;
   CUDA_TRY(cudaEventRecord(qp->ev0, st));
-  CUDA_TRY(cudaMemsetAsync(qp->K, 0, bn * qp->numax * qp->nx * sizeof(double), st));
-  CUDA_TRY(cudaMemsetAsync(qp->kff, 0, bn * qp->numax * sizeof(double), st));
+  CUDA_TRY(cudaMemsetAsync(v.K, 0, bn * v.numax * v.nx * sizeof(double), st));
+  CUDA_TRY(cudaMemsetAsync(v.kff, 0, bn * v.numax * sizeof(double), st));
   launch_riccati(v, st);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaEventRecord(qp->ev1, st));
@@ -311,23 +274,24 @@ int b200sqp_qp_download(b200sqp_qp qp, double* dx, double* du, double* K, double
   if ((P || p) && !qp->keptP) return fail(B200SQP_ESTATE, "qp_download: cost-to-go requested but solve ran with keep_P = 0");
   CUDA_TRY(cudaSetDevice(qp->device));
   CUDA_TRY(cudaDeviceSynchronize());
-  const size_t bn = static_cast<size_t>(qp->B) * qp->N, bn1 = static_cast<size_t>(qp->B) * (qp->N + 1);
-  const int nx = qp->nx, nm = qp->numax;
+  const b200sqp::QpDeviceView& v = qp->v;
+  const size_t bn = static_cast<size_t>(v.B) * v.N, bn1 = static_cast<size_t>(v.B) * (v.N + 1);
+  const int nx = v.nx, nm = v.numax;
   auto dn = [&](double* h, const double* d, size_t n) { return h ? cudaMemcpy(h, d, n * sizeof(double), cudaMemcpyDeviceToHost) : cudaSuccess; };
-  CUDA_TRY(dn(dx, qp->dx, bn1 * nx));
-  CUDA_TRY(dn(du, qp->du, bn * nm));
-  CUDA_TRY(dn(K, qp->K, bn * nm * nx));
-  CUDA_TRY(dn(k, qp->kff, bn * nm));
-  CUDA_TRY(dn(P, qp->P, bn1 * nx * nx));
-  CUDA_TRY(dn(p, qp->p, bn1 * nx));
-  std::vector<int> st(qp->B);
-  CUDA_TRY(cudaMemcpy(st.data(), qp->status, qp->B * sizeof(int), cudaMemcpyDeviceToHost));
+  CUDA_TRY(dn(dx, v.dx, bn1 * nx));
+  CUDA_TRY(dn(du, v.du, bn * nm));
+  CUDA_TRY(dn(K, v.K, bn * nm * nx));
+  CUDA_TRY(dn(k, v.kff, bn * nm));
+  CUDA_TRY(dn(P, v.P, bn1 * nx * nx));
+  CUDA_TRY(dn(p, v.p, bn1 * nx));
+  std::vector<int> st(v.B);
+  CUDA_TRY(cudaMemcpy(st.data(), v.status, v.B * sizeof(int), cudaMemcpyDeviceToHost));
   int bad = 0;
-  for (int i = 0; i < qp->B; ++i) {
+  for (int i = 0; i < v.B; ++i) {
     if (status) status[i] = st[i];
     bad += st[i] != 0;
   }
-  if (bad) return fail(B200SQP_EQP, "[b200sqp] Failed to solve QP for %d of %d instances", bad, qp->B);
+  if (bad) return fail(B200SQP_EQP, "[b200sqp] Failed to solve QP for %d of %d instances", bad, v.B);
   return 0;
 }
 

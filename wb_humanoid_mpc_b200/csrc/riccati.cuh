@@ -49,6 +49,37 @@ struct QpDeviceView {
   int skipStride;
 };
 
+// The granularity of a batch array: one row per instance, per node (N + 1 per instance) or per stage (N per instance), or one block for the
+// whole handle.  batchRows: the rows of B instances of `nodes` nodes each.
+enum RowKind { ROW_INST, ROW_NODE, ROW_STAGE, ROW_HANDLE };
+__host__ __device__ inline size_t batchRows(RowKind k, size_t B, int nodes) {
+  return k == ROW_INST ? B : k == ROW_NODE ? B * nodes : k == ROW_STAGE ? B * (nodes - 1) : 1;
+}
+
+// The arrays of a QP batch, in allocation order: f(field, row kind, width in elements).  withP: the cost-to-go matrices, which only a solve
+// that keeps them needs.
+template <class F>
+void forEachQpArray(QpDeviceView& v, bool withP, F&& f) {
+  const int nx = v.nx, nm = v.numax;
+  f(v.A, ROW_STAGE, nx * nx);
+  f(v.Bm, ROW_STAGE, nx * nm);
+  f(v.b, ROW_STAGE, nx);
+  f(v.Q, ROW_NODE, nx * nx);
+  f(v.S, ROW_STAGE, nm * nx);
+  f(v.R, ROW_STAGE, nm * nm);
+  f(v.q, ROW_NODE, nx);
+  f(v.r, ROW_STAGE, nm);
+  f(v.dx0, ROW_INST, nx);
+  f(v.nu, ROW_STAGE, 1);
+  f(v.K, ROW_STAGE, nm * nx);
+  f(v.kff, ROW_STAGE, nm);
+  f(v.p, ROW_NODE, nx);
+  if (withP) f(v.P, ROW_NODE, nx * nx);
+  f(v.dx, ROW_NODE, nx);
+  f(v.du, ROW_STAGE, nm);
+  f(v.status, ROW_INST, 1);
+}
+
 __host__ __device__ inline int even_up(int n) { return (n + 1) & ~1; }
 
 struct RicLayout {

@@ -41,12 +41,8 @@ __global__ void __launch_bounds__(128) mrt_check_kernel(const double* robot, int
 __global__ void __launch_bounds__(64) mrt_dev_out_kernel(const double* jout, const double* xout, const double* uout, const int* modeIn, const int* gtab,
                                                          const int* slotInst, const int* st, int B, int nxAbi, MrtDevOut o) {
   const int s = blockIdx.x;
-  int first = 0, count = B;
-  if (gtab) {
-    const int g = fleetGroupOf(gtab, s);
-    first = gtab[2 + 3 * g];
-    count = gtab[3 + 3 * g];
-  }
+  const FleetSlot sl = fleetSlot(gtab, B, 1, s);   // (one row per slot: no node rows)
+  const int first = sl.first, count = sl.count;
   const size_t i = slotInst ? slotInst[s] : s, k = s - first;
   const int code = st ? st[i] : 0;
   const double nan = __longlong_as_double(0x7ff8000000000000LL);
@@ -72,15 +68,10 @@ __global__ void __launch_bounds__(64) mrt_dev_out_kernel(const double* jout, con
 __global__ void __launch_bounds__(128) plan_gather_kernel(WbDev base, int capNodes, const int* gtab, const int* slotInst, int maxNodes, int nxAbi,
                                                           double* x, double* u, double* K, int* status) {
   const int s = blockIdx.y, r = blockIdx.x;
-  int n = capNodes, first = 0;
-  if (gtab) {
-    const int g = fleetGroupOf(gtab, s);
-    n = gtab[1 + 3 * g];
-    first = gtab[2 + 3 * g];
-  }
+  const FleetSlot sl = fleetSlot(gtab, gridDim.y, capNodes, s);
+  const int n = sl.n;
   const size_t i = slotInst ? slotInst[s] : s;
-  const size_t node = static_cast<size_t>(first) * capNodes + static_cast<size_t>(s - first) * n + r;
-  const size_t stage = static_cast<size_t>(first) * (capNodes - 1) + static_cast<size_t>(s - first) * (n - 1) + r;
+  const size_t node = sl.node + r, stage = sl.stage + r;
   if (x) {
     double* o = x + (i * maxNodes + r) * nxAbi;
     for (int j = threadIdx.x; j < nxAbi; j += blockDim.x) o[j] = r < n ? base.x[node * NX + j] : 0.0;

@@ -5,6 +5,7 @@
 //   carry    the iterate of every view -> the builder's caller-order previous solution (per-instance length, rows strided by the capacity);
 //   permute  caller order <-> slot order for the roll-out / joint-action inputs and outputs and the simulated state.
 #pragma once
+#include "wb_batch.cuh"
 #include "wb_builder.cuh"
 
 namespace b200sqp {
@@ -58,6 +59,25 @@ HD int fleetGroupOf(const int* gtab, int s) {
   while (g + 1 < gtab[0] && s >= gtab[2 + 3 * (g + 1)]) ++g;
   return g;
 }
+// slot s of a batch of B instances allocated at capNodes nodes each: its group's node count, first slot and size (gtab null: a plain handle,
+// one group of B instances at capNodes nodes), and the slot's first node and stage rows in the allocation (groupView's rows, then the slot's
+// position in its group)
+struct FleetSlot {
+  int n, first, count;
+  size_t node, stage;
+};
+HD FleetSlot fleetSlot(const int* gtab, int B, int capNodes, int s) {
+  FleetSlot r{capNodes, 0, B, 0, 0};
+  if (gtab) {
+    const int g = fleetGroupOf(gtab, s);
+    r.n = gtab[1 + 3 * g];
+    r.first = gtab[2 + 3 * g];
+    r.count = gtab[3 + 3 * g];
+  }
+  r.node = batchRows(ROW_NODE, r.first, capNodes) + batchRows(ROW_NODE, s - r.first, r.n);
+  r.stage = batchRows(ROW_STAGE, r.first, capNodes) + batchRows(ROW_STAGE, s - r.first, r.n);
+  return r;
+}
 
 #ifdef __CUDACC__
 // one CTA; dynamic shared memory: nBins ints
@@ -84,11 +104,9 @@ __global__ void fleet_partition_kernel(const BldScratch* sc, int B, int nBins, i
 __global__ void __launch_bounds__(128) fleet_carry_kernel(WbDev base, int capNodes, const int* gtab, const int* slotInst, double* prevX, double* prevU,
                                                           double* prevT, uint8_t* prevE, int* prevLen) {
   const int s = blockIdx.x;
-  const int g = fleetGroupOf(gtab, s);
-  const int n = gtab[1 + 3 * g], first = gtab[2 + 3 * g];
-  const int i = slotInst[s];
-  const size_t node0 = static_cast<size_t>(first) * capNodes + static_cast<size_t>(s - first) * n;            // first node of the slot
-  const size_t stage0 = static_cast<size_t>(first) * (capNodes - 1) + static_cast<size_t>(s - first) * (n - 1);
+  const FleetSlot sl = fleetSlot(gtab, gridDim.x, capNodes, s);
+  const int n = sl.n, i = slotInst[s];
+  const size_t node0 = sl.node, stage0 = sl.stage;
   const size_t dst = static_cast<size_t>(i) * capNodes;
   for (size_t j = threadIdx.x; j < static_cast<size_t>(n) * NX; j += blockDim.x) prevX[dst * NX + j] = base.x[node0 * NX + j];
   for (size_t j = threadIdx.x; j < static_cast<size_t>(n - 1) * NU; j += blockDim.x) prevU[dst * NU + j] = base.u[stage0 * NU + j];
