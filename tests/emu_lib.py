@@ -31,6 +31,14 @@ def dyn(desc, x, u, deriv=True):
     return xd, G.T.copy()
 
 
+def penalty(kind, mu, delta, h):
+    """(v, d1, d2) of the device's penRelaxed (kind "relaxed") or penPwPoly (kind "pwpoly") at h"""
+    out = np.zeros(3)
+    rc = lib().emu_penalty(C.c_int({"relaxed": 0, "pwpoly": 1}[kind]), C.c_double(mu), C.c_double(delta), C.c_double(h), _p(out))
+    assert rc == 0
+    return tuple(float(v) for v in out)
+
+
 def lq_node(desc, x, u, xnext, xref, dt, contact, swing, impact, arm_phase, mode=0):
     """mode 0: one-pass K1b schedule; 1 / 2: the CUDA schedules (lu + part 1 + part 2; 2 = Q accumulated in place)."""
     NX, NU, NT = 58, 35, 23
