@@ -50,7 +50,9 @@ const char* b200sqp_version(void);
  * ------------------------------------------------------------------------------------------------------------------ */
 typedef struct b200sqp_qp_t* b200sqp_qp;
 
-/* HpipmInterface::HpipmInterface(OcpSize) / resize(): allocate device storage for `batch` problems of N stages. */
+/* HpipmInterface::HpipmInterface(OcpSize) / resize(): allocate device storage for `batch` problems of N stages.
+ * Accepts 0 < nx <= 64 and 0 < nu_max <= 32 whose Riccati working set fits one block's shared memory in both kernel variants (1948 of the
+ * 2048 pairs; the largest nu_max for nx = 64 is 15); B200SQP_EINVAL otherwise. */
 int b200sqp_qp_create(int device, int batch, int N, int nx, int nu_max, b200sqp_qp* out);
 void b200sqp_qp_destroy(b200sqp_qp qp);
 

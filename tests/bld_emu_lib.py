@@ -325,6 +325,20 @@ def fleet_slots(groups, B, cap):
     return out
 
 
+RIC_FIELDS = ("pq", "ab", "w", "y", "rs", "linv", "vec", "total", "kout")
+
+
+def riccati_layout(nx, nm):
+    """the shared-memory layouts of the generic Riccati kernels at (nx, nm) -> dict(one=..., cluster=...) of RIC_FIELDS (doubles), with
+    one_doubles / cluster_doubles (the dynamic shared memory of each kernel), lx / lm (the one-CTA kernel's leading dimensions), supported
+    (b200sqp_qp_create accepts the size) and limit (its byte limit)"""
+    out = np.zeros(24, np.int64)
+    lib().emu_riccati_layout(C.c_int(nx), C.c_int(nm), _i64(out))
+    v = [int(x) for x in out]
+    return dict(one=dict(zip(RIC_FIELDS, v[0:9])), cluster=dict(zip(RIC_FIELDS, v[9:18])), one_doubles=v[18], cluster_doubles=v[19], lx=v[20],
+                lm=v[21], supported=bool(v[22]), limit=v[23])
+
+
 def base_velocity(model, x):
     """bldCenBaseVelocity of centroidal states x [n, CNX] -> [n, 6]"""
     from wb_humanoid_mpc_b200 import abi

@@ -1,5 +1,6 @@
 // DEVELOPMENT HARNESS (tests only, never linked into libb200sqp.so): the device builder (wb_builder.cuh), the fleet's partition and slot helper
-// (wb_fleet.cuh) and the batch layout (wb_batch.cuh) executed on the CPU.  One context holds B instances' builder state the way the handle's batch
+// (wb_fleet.cuh), the batch layout (wb_batch.cuh) and the shared-memory layouts of the Riccati kernels (riccati.cuh, riccati_cluster.cuh) executed
+// on the CPU.  One context holds B instances' builder state the way the handle's batch
 // allocation does, and emu_bld_build runs the work items in the order b200sqp_build_instances launches its kernels, every loop in reverse so that
 // an order dependence shows as a mismatch.
 // Built into tests/emu/libbldemu.so by tests/bld_emu_lib.py.  The product has no CPU path.
@@ -11,6 +12,7 @@
 #include <vector>
 
 #include "../../wb_humanoid_mpc_b200/csrc/cen_host.cuh"
+#include "../../wb_humanoid_mpc_b200/csrc/riccati_cluster.cuh"
 #include "../../wb_humanoid_mpc_b200/csrc/wb_fleet.cuh"
 
 using namespace b200sqp;
@@ -583,6 +585,25 @@ int emu_cen_base_velocity(const b200sqp_model_desc* d, const b200sqp_cen_desc* c
   static CenKin k;
   for (int i = n - 1; i >= 0; --i) bldCenBaseVelocity(m.ocp.kin, x + static_cast<size_t>(i) * NX, total_mass, k, bv + 6 * i);
   return 0;
+}
+
+// The shared-memory layouts of the generic Riccati kernels at (nx, nm), in doubles: out[0..9) riccati_layout_padded (the one-CTA kernel) and
+// out[9..18) riccati_layout (the cluster kernel), each as {pq, ab, w, y, rs, linv, vec, total, kout}; out[18] riccati_smem_doubles and
+// out[19] riccati_cluster_smem_doubles; out[20], out[21] the one-CTA kernel's leading dimensions ric_pad(nx), ric_pad(nm); out[22] whether
+// b200sqp_qp_create accepts the size (riccati_sizes_supported); out[23] the byte limit it applies.
+void emu_riccati_layout(int nx, int nm, long long* out) {
+  const RicLayout ls[2] = {riccati_layout_padded(nx, nm), riccati_layout(nx, nm)};
+  for (int i = 0; i < 2; ++i) {
+    const RicLayout& L = ls[i];
+    const int f[9] = {L.pq, L.ab, L.w, L.y, L.rs, L.linv, L.vec, L.total, L.kout};
+    for (int j = 0; j < 9; ++j) out[9 * i + j] = f[j];
+  }
+  out[18] = static_cast<long long>(riccati_smem_doubles(nx, nm));
+  out[19] = static_cast<long long>(riccati_cluster_smem_doubles(nx, nm));
+  out[20] = ric_pad(nx);
+  out[21] = ric_pad(nm);
+  out[22] = riccati_sizes_supported(nx, nm);
+  out[23] = static_cast<long long>(RIC_SMEM_BYTES_MAX);
 }
 
 }  // extern "C"

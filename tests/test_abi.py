@@ -20,6 +20,12 @@ def test_header_and_loader_agree():
     assert header_symbols() == sorted(lib.EXPORTED_SYMBOLS)
 
 
+def test_return_codes_match_header():
+    text = (ROOT / "include" / "b200sqp.h").read_text()
+    codes = {m[0]: int(m[1]) for m in re.findall(r"#define B200SQP_(E[A-Z]+)\s+(-?\d+)", text)}
+    assert codes == {name: getattr(lib, name) for name in ("EINVAL", "ENODEV", "ENOMEM", "EQP", "ESTATE")}
+
+
 def test_library_exports_every_declared_symbol():
     L = lib.lib()
     for name in header_symbols():

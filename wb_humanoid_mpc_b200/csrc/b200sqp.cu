@@ -186,8 +186,10 @@ int b200sqp_qp_create(int device, int batch, int N, int nx, int nu_max, b200sqp_
   if (!out || batch <= 0 || N <= 0 || nx <= 0 || nx > 64 || nu_max <= 0 || nu_max > 32)
     return fail(B200SQP_EINVAL, "qp_create: need batch,N > 0, 0 < nx <= 64 and 0 < nu_max <= 32 (got %d,%d,%d,%d)", batch, N, nx, nu_max);
   if (int rc = select_device(device)) return rc;
-  const size_t smem = b200sqp::riccati_smem_doubles(nx, nu_max) * sizeof(double);
-  if (smem > 227 * 1024) return fail(B200SQP_EINVAL, "qp_create: nx=%d nu_max=%d needs %zu B shared memory (> 227 KB)", nx, nu_max, smem);
+  if (!b200sqp::riccati_sizes_supported(nx, nu_max))
+    return fail(B200SQP_EINVAL, "qp_create: nx=%d nu_max=%d needs %zu B (one-CTA kernel) and %zu B (cluster kernel) of shared memory (limit %zu B)",
+                nx, nu_max, b200sqp::riccati_smem_doubles(nx, nu_max) * sizeof(double),
+                b200sqp::riccati_cluster_smem_doubles(nx, nu_max) * sizeof(double), b200sqp::RIC_SMEM_BYTES_MAX);
   b200sqp_qp_t* qp = new (std::nothrow) b200sqp_qp_t;
   if (!qp) return fail(B200SQP_ENOMEM, "host allocation failed");
   qp->device = device;

@@ -84,14 +84,19 @@ __host__ __device__ inline int even_up(int n) { return (n + 1) & ~1; }
 
 struct RicLayout {
   int pq, ab, w, y, rs, linv, vec, total;  // sizes in doubles
+  int kout;   // offset of [K | k] inside W
 };
 // Vectors ride along as extra matrix columns so that every matrix-vector product is folded into a tensor-core GEMM:
 //   PQ = [P | p] (nx x (nx+1)),  AB = [A | b | B] (nx x (nx+1+nm)),  Y = [S | r] (nm x (nx+1))
+// The scratch W first holds P [A | b | B] (the shape of AB), later [Yl | yl] (nm x (nx+1), at the leading dimension of Y) followed by
+// [K | k] (nm x (nx+1), leading dimension nm): it is sized for the larger of the two uses (the second one, roughly, once nm >= nx).
 __host__ __device__ inline RicLayout riccati_layout(int nx, int nm) {
   RicLayout L;
   L.pq = even_up(nx * (nx + 1));
   L.ab = even_up(nx * (nx + 1 + nm));
-  L.w = L.ab;
+  L.kout = even_up(nm * (nx + 1));
+  const int ylk = L.kout + even_up(nm * (nx + 1));   // [Yl | yl] and [K | k]
+  L.w = ylk > L.ab ? ylk : L.ab;
   L.y = even_up(nm * (nx + 1));
   L.rs = even_up(nm * nm);
   L.linv = even_up(nm * nm);
@@ -108,7 +113,9 @@ __host__ __device__ inline RicLayout riccati_layout_padded(int nx, int nm) {
   RicLayout L;
   L.pq = even_up(lx * (nx + 1));
   L.ab = even_up(lx * (nx + 1 + nm));
-  L.w = L.ab;
+  L.kout = even_up(lm * (nx + 1));
+  const int ylk = L.kout + even_up(nm * (nx + 1));   // [Yl | yl] and [K | k]
+  L.w = ylk > L.ab ? ylk : L.ab;
   L.y = even_up(lm * (nx + 1));
   L.rs = even_up(lm * nm);
   L.linv = even_up(lm * nm);
@@ -250,7 +257,7 @@ __global__ void __launch_bounds__(256, 1) riccati_kernel(QpDeviceView v) {
       RIC_TICK(6)
       // ---- [Yl | yl] = L^-1 [S~ | r~] (into W) ---------------------------------------------------------------------------------
       double* Yl = W;
-      double* Kout = W + even_up(lm * nx1);   // [K | k] keeps the dense leading dimension nm of its destination in HBM
+      double* Kout = W + L.kout;   // [K | k] keeps the dense leading dimension nm of its destination in HBM
       par_mma_gemm<false, false, 4>(P, nu, nx1, nu, 1.0, Linv, lm, Yk, lm, Yl, lm);
       __syncthreads();
     RIC_TICK(8)

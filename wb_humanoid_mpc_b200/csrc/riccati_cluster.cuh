@@ -24,6 +24,18 @@ __host__ __device__ inline size_t riccati_cluster_smem_doubles(int nx, int numax
   return static_cast<size_t>(L.total) + L.rs + L.y;
 }
 
+// The dynamic shared memory one block of a generic Riccati kernel may take: the 227 KB a block can opt into on sm_90, less the kernels' 16
+// bytes of static shared memory (the `ok` flag, padded).
+constexpr size_t RIC_SMEM_BYTES_MAX = 227 * 1024 - 16;
+// The sizes b200sqp_qp_create accepts.  nu_max <= 32: warp_chol_inverse keeps one column per lane, and the forward sweep has 8 lanes per row of
+// u in a 256-thread block; nx <= 64: 4 lanes per row of x.  launch_riccati picks the one-CTA or the cluster kernel by the batch size alone, so
+// the layouts of both must fit.
+__host__ __device__ inline bool riccati_sizes_supported(int nx, int nm) {
+  if (nx <= 0 || nx > 64 || nm <= 0 || nm > 32) return false;
+  return riccati_smem_doubles(nx, nm) * sizeof(double) <= RIC_SMEM_BYTES_MAX &&
+         riccati_cluster_smem_doubles(nx, nm) * sizeof(double) <= RIC_SMEM_BYTES_MAX;
+}
+
 __device__ __forceinline__ int sliceLo(int n, int r) { return (n * r) / RC; }
 
 // copy columns [c0, c1) of a column-major (rows x *) block from the local buffer to the same place in every peer's buffer
@@ -129,7 +141,7 @@ __global__ void __cluster_dims__(RC, 1, 1) __launch_bounds__(256, 1) riccati_clu
     for (int i = bc0 + threadIdx.x; i < bc1; i += blockDim.x) Rk[i + i * nm] += v.reg;
     __syncthreads();
     double* Yl = W;
-    double* Kout = W + even_up(nm * nx1);
+    double* Kout = W + L.kout;
     if (nu > 0) {
       // ---- all-gather R~ and [S~ | r~] in one exchange, factorise and form Yl = L^-1 [S~ | r~] everywhere (identical arithmetic) ---------------
       for (int t = threadIdx.x; t < nm * (bc1 - bc0); t += blockDim.x) Rg[(t % nm) + nm * (bc0 + t / nm)] = Rk[(t % nm) + nm * (bc0 + t / nm)];

@@ -23,6 +23,9 @@ dp = C.POINTER(C.c_double)
 ip = C.POINTER(C.c_int32)
 u8p = C.POINTER(C.c_uint8)
 
+# the return codes of include/b200sqp.h (B200SQP_E*; tests/test_abi.py checks them against the header)
+EINVAL, ENODEV, ENOMEM, EQP, ESTATE = -1, -2, -3, -4, -5
+
 
 class B200SqpError(RuntimeError):
     def __init__(self, code, msg):

@@ -69,7 +69,7 @@ class BatchedQp:
         p = np.zeros((Bn, N + 1, nx)) if self._keptP else None
         status = np.zeros(Bn, dtype=np.int32)
         rc = _l.lib().b200sqp_qp_download(self._h, _p(dx), _p(du), _p(K), _p(k), _p(P), _p(p), status.ctypes.data_as(_l.ip))
-        if rc != 0 and (raise_on_failure or rc != -4):   # -4 = B200SQP_EQP: every array has been filled, status says which instances failed
+        if rc != 0 and (raise_on_failure or rc != _l.EQP):   # EQP: every array has been filled, status says which instances failed
             _l.check(rc)
         out = dict(dx=dx, du=du, K=np.swapaxes(K, -1, -2).copy(), k=k, status=status)
         if self._keptP:
