@@ -98,7 +98,10 @@ int launch_riccati(const b200sqp::QpDeviceView& v, cudaStream_t st) {
   } else {
     const char* legacy = std::getenv("B200SQP_K2_LEGACY");
     if (wb && !(legacy && legacy[0] == '1')) {
-      b200sqp::ricwb::riccati_bwd_kernel<<<v.B, b200sqp::ricwb::BWD_THREADS, b200sqp::ricwb::BWD_SMEM_BYTES, st>>>(v);
+      // two instances per CTA (c and c + ceil(B / 2)) once the batch is larger than the SM count, so that it runs in one wave up to twice
+      // that; one per CTA below, so that no SM idles
+      const int pairOff = v.B > sms ? (v.B + 1) / 2 : 0;
+      b200sqp::ricwb::riccati_bwd_kernel<<<pairOff ? pairOff : v.B, b200sqp::ricwb::BWD_THREADS, b200sqp::ricwb::BWD_SMEM_BYTES, st>>>(v, pairOff);
       b200sqp::ricwb::riccati_fwd_kernel<<<v.B, b200sqp::ricwb::FWD_THREADS, b200sqp::ricwb::FWD_SMEM_BYTES, st>>>(v);
       return 2;
     }

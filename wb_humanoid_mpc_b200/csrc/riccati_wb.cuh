@@ -1,15 +1,20 @@
 // K2 for the whole-body sizes (nx = 58, nu_max = 23), large batches: the Riccati recursion of HpipmInterface::solve
 // (lib/ocs2_ros2/ocs2_sqp/hpipm_catkin/src/HpipmInterface.cpp:166-455) as TWO kernels.
 //
-//   riccati_bwd_kernel  backward factorisation, one persistent CTA per instance (216 KB of shared memory: one CTA per SM).
-//                       Nine warps: warps 0-7 run the fp64 tensor-path contractions (DMMA m8n8k4), warp 8 is a helper warp that
-//                       (a) streams the next stage record with cp.async.bulk + an mbarrier: one elected lane arms the barrier and issues SIX bulk
-//                       copies (A, b, B, Q, q, S land densely, leading dimension 58 / 23, exactly as they lie in HBM; the 552 doubles of r and R,
-//                       whose HBM addresses are only 8-byte aligned, ride as cp.async), (b) factorises R~ = L L' and inverts L, register resident, WHILE the
-//                       GEMM warps form Q~ and S~ (the factorisation only needs R~, which is formed first and handed over through a named
-//                       barrier), (c) writes the cost-to-go out when it is kept.
+//   riccati_bwd_kernel  backward factorisation, one persistent CTA of two independent LANES, each running one instance (112 KB of shared
+//                       memory per lane, one CTA per SM).  The sweep is bound by latency (the factorisation chain, barriers, fragment loads), so
+//                       two instances side by side on one SM overlap: a batch of up to twice the SM count runs in one wave.  Batches no larger than
+//                       the SM count run one lane per CTA, so that no SM idles.  A lane is five warps: four GEMM warps run the fp64 tensor-path
+//                       contractions (DMMA m8n8k4) and one helper warp
+//                       (a) streams the next stage's [A | b | B] with cp.async.bulk + an mbarrier once this stage's last read of it is done
+//                       (it lands densely, leading dimension 58, exactly as it lies in HBM), prefetches Q, q, S, r of the next stage into L2 and
+//                       R as 8-byte cp.async (its HBM address is only 8-byte aligned), (b) factorises R~ = L L' and inverts L, register resident,
+//                       WHILE the GEMM warps form Q~ and S~ (the factorisation only needs R~, which is formed first and handed over through a
+//                       named barrier), (c) writes the cost-to-go out when it is kept.  Q, q, S, r are never staged in shared memory: they are
+//                       the addends of the epilogues that form Q~ and [S~ | r~], read from global memory.
 //                       Per stage:  W = P [A | b | B], W_b += p           (P is kept as its lower triangle: the operand loads pick (max, min))
-//                                   R~ = R + B'W_B  ->  warp 8: L, L^-1   ||  Q~ = Q + A'W_A (lower tiles only), [S~ | r~] = [S | r] + B'[W_A | v]
+//                                   R~ = R + B'W_B  ->  helper: L, L^-1   ||  Q~ = Q + A'W_A (lower tiles only, over the dead P),
+//                                                                             [S~ | r~] = [S | r] + B'[W_A | v] (over the dead W_B)
 //                                   Yl = L^-1 [S~ | r~]
 //                                   [P | p] = [Q~ | q~] - Yl'Yl (lower tiles only), [K | k] = -L^-T Yl
 //   riccati_fwd_kernel  forward substitution, one small CTA per instance (two resident per SM, so the whole batch is in flight and the
@@ -45,16 +50,29 @@ namespace ricwb {
 
 constexpr int NXR = 58, NX1R = 59, NMR = 23;
 constexpr int LWR = 60, LMR = 28;                 // leading dimensions of the operands the kernel produces itself: = 4 (mod 8), conflict-free DMMA fragment loads
-constexpr int GEMM_WARPS = 8, BWD_THREADS = 32 * (GEMM_WARPS + 1);
-constexpr int PQ_D = NXR * NX1R + 2;              // [P | p], dense (ld 58), lower triangle of P valid
+constexpr int LANES = 2, LANE_GEMM_WARPS = 4;
+constexpr int LANE_THREADS = 32 * (LANE_GEMM_WARPS + 1), BWD_THREADS = LANES * LANE_THREADS;
+constexpr int PQ_D = NXR * NX1R + 2;              // [P | p], dense (ld 58), lower triangle of P valid; [Q~ | q~] once W is complete
 constexpr int AB_D = NXR * (NX1R + NMR);          // [A | b | B], dense (ld 58): a 58 x 82 matrix
-constexpr int W_D = LWR * (NX1R + NMR);           // W (ld 60); later Yl (ld 28) and [K | k] (ld 23)
-constexpr int Y_D = NMR * NX1R + 1;               // [S | r], dense (ld 23)
-constexpr int R_D = LMR * NMR;                    // R, L^-1 (ld 28)
+constexpr int W_D = LWR * (NX1R + NMR);           // W (ld 60); later Yl (ld 28), [K | k] (ld 23) and [S~ | r~] (ld 23)
+constexpr int R_D = LMR * NMR;                    // 23 x 23 at ld 28
 constexpr int YL_D = LMR * NX1R;
 constexpr int KOUT_OFF = YL_D;                    // [K | k] behind Yl inside the W region
-constexpr int BWD_SMEM_D = 2 * PQ_D + 2 * AB_D + W_D + 2 * Y_D + 3 * R_D + 8;
+constexpr int Y_OFF = LWR * NX1R;                 // [S~ | r~] in the columns of W_B, dead once R~ is formed
+// the shared memory of one lane (doubles); the two lanes' maps follow each other, then one mbarrier per lane
+constexpr int PQ_OFF = 0;
+constexpr int AB_OFF = PQ_OFF + PQ_D;
+constexpr int W_OFF = AB_OFF + AB_D;
+constexpr int RT_OFF = W_OFF + W_D;               // R~, overwritten by L^-1 (the helper warp holds R~ in registers by then)
+constexpr int RIN_OFF = RT_OFF + R_D;             // R, landing buffer of the cp.async (read by the epilogue of R~)
+constexpr int LANE_D = RIN_OFF + R_D;
+constexpr int BWD_SMEM_D = LANES * LANE_D + LANES;
 constexpr size_t BWD_SMEM_BYTES = static_cast<size_t>(BWD_SMEM_D) * 8;
+constexpr size_t BWD_STATIC_SMEM_BYTES = 16;   // the lanes' `ok` flags, as ptxas allots them
+static_assert(PQ_D % 2 == 0 && AB_D % 2 == 0 && W_D % 2 == 0 && R_D % 2 == 0, "bulk-copy targets and lane bases start on 16-byte boundaries");
+static_assert(YL_D <= KOUT_OFF && KOUT_OFF + NMR * NX1R <= Y_OFF, "Yl and [K | k] stay below the W_B columns that hold [S~ | r~]");
+static_assert(Y_OFF + NMR * NX1R <= W_D, "[S~ | r~] (ld 23) fits the W_B columns");
+static_assert(BWD_SMEM_BYTES + BWD_STATIC_SMEM_BYTES <= 227 * 1024, "two lanes fit a block's opt-in shared memory on sm_90");
 
 // ---- mbarrier / bulk-copy primitives (sm_90+; SASS: SYNCS.*, UBLKCP) -------------------------------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return static_cast<unsigned>(__cvta_generic_to_shared(p)); }
@@ -84,6 +102,11 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned by
                "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// global -> L2 prefetch (bytes: a multiple of 16; address 16-byte aligned), and of the one cache line that holds address p
+__device__ __forceinline__ void bulk_prefetch_l2(const void* src, unsigned bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // generic-proxy accesses of this thread before, async-proxy accesses after (a buffer read with ld.shared is about to be refilled by a bulk copy)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_arrive(int id, int count) { asm volatile("barrier.cta.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
@@ -94,7 +117,10 @@ __device__ __forceinline__ void named_sync(int id, int count) { asm volatile("ba
 // KC > 0: contraction length known at compile time (the k loop unrolls completely and the scheduler hoists the fragment loads).
 // NG is a compile-time count (mma_item dispatches on the number of tiles) so that the unrolled DMMA stream carries no per-tile branches.
 // SYM_A (only with !TRANS_A, M = K): A is symmetric and only its lower triangle is valid: element (m, k) is read from (max, min).
-// vadd != nullptr: column vcol of the result additionally gets the vector vadd (W_b = P b + p without a separate pass).
+// vadd != nullptr: without ACC, column vcol of the result additionally gets the vector vadd (W_b = P b + p without a separate pass); with ACC,
+// vadd is the addend of column vcol in place of Cin's column (C-in [Q | q] from Q and q, which lie apart in HBM).
+// ACC: C = alpha * op(A) * B + Cin, Cin = C unless given (leading dimension ldcin).  The addends are loaded before the contraction, so that the
+// latency of a global Cin hides behind it.
 // PERM_A / PERM_B: the operand has leading dimension 58 with the contraction index running fastest (A' stored K x M, or B): lane group fr then
 // takes row / column perm8(fr) = (0, 2, 4, 6, 1, 3, 5, 7)[fr] of the tile instead of fr.  A half-warp's fragment load touches the doubles
 // {k + 58 n : k = 0..3, n = four rows / columns}: with n = 0, 1, 2, 3 the bank offsets 10 n (mod 16) = 0, 10, 4, 14 make the 4-wide runs of
@@ -104,7 +130,7 @@ __device__ __forceinline__ int perm8(int j) { return j < 4 ? 2 * j : 2 * (j - 4)
 template <bool TRANS_A, bool ACC, int NG, int KC, bool SYM_A, bool PERM_A, bool PERM_B>
 __device__ __forceinline__ void mma_item_ng(int lane, int M, int N, int Krt, double alpha, const double* __restrict__ A, int lda, int tm,
                                             const double* __restrict__ B, int ldb, const int* tn, double* __restrict__ C, int ldc,
-                                            const double* __restrict__ vadd, int vcol) {
+                                            const double* __restrict__ vadd, int vcol, const double* __restrict__ Cin, int ldcin) {
   const int K = KC ? KC : Krt;
   const int fr = lane >> 2, fk = lane & 3;
   const int Kmain = K & ~3;
@@ -125,6 +151,17 @@ __device__ __forceinline__ void mma_item_ng(int lane, int M, int N, int Krt, dou
     bok[g] = bn < N;
     Bp[g] = B + fk + (bok[g] ? bn : 0) * ldb;
     c0[g] = c1[g] = 0.0;
+  }
+  double in0[NG], in1[NG];
+  if (ACC) {
+    const double* ci = Cin ? Cin : C;
+    const int ldi = Cin ? ldcin : ldc;
+#pragma unroll
+    for (int g = 0; g < NG; ++g) {
+      const int cn0 = (tn[g] << 3) + cj0, cn1 = (tn[g] << 3) + cj1;
+      in0[g] = (arok && cn0 < N) ? ((vadd && cn0 == vcol) ? vadd[ar] : ci[ar + cn0 * ldi]) : 0.0;
+      in1[g] = (arok && cn1 < N) ? ((vadd && cn1 == vcol) ? vadd[ar] : ci[ar + cn1 * ldi]) : 0.0;
+    }
   }
 #pragma unroll
   for (int k0 = 0; k0 < Kmain; k0 += 4) {
@@ -160,16 +197,14 @@ __device__ __forceinline__ void mma_item_ng(int lane, int M, int N, int Krt, dou
     for (int g = 0; g < NG; ++g) {
       const int cn0 = (tn[g] << 3) + cj0, cn1 = (tn[g] << 3) + cj1;
       if (cn0 < N) {
-        double* c = &C[ar + cn0 * ldc];
-        double r = ACC ? fma(alpha, c0[g], *c) : alpha * c0[g];
-        if (vadd && cn0 == vcol) r += vadd[ar];
-        *c = r;
+        double r = ACC ? fma(alpha, c0[g], in0[g]) : alpha * c0[g];
+        if (!ACC && vadd && cn0 == vcol) r += vadd[ar];
+        C[ar + cn0 * ldc] = r;
       }
       if (cn1 < N) {
-        double* c = &C[ar + cn1 * ldc];
-        double r = ACC ? fma(alpha, c1[g], *c) : alpha * c1[g];
-        if (vadd && cn1 == vcol) r += vadd[ar];
-        *c = r;
+        double r = ACC ? fma(alpha, c1[g], in1[g]) : alpha * c1[g];
+        if (!ACC && vadd && cn1 == vcol) r += vadd[ar];
+        C[ar + cn1 * ldc] = r;
       }
     }
   }
@@ -177,12 +212,16 @@ __device__ __forceinline__ void mma_item_ng(int lane, int M, int N, int Krt, dou
 template <bool TRANS_A, bool ACC, int NG, int KC, bool SYM_A = false, bool PERM_A = false, bool PERM_B = false>
 __device__ __forceinline__ void mma_item(int lane, int M, int N, int Krt, double alpha, const double* __restrict__ A, int lda, int tm,
                                          const double* __restrict__ B, int ldb, const int (&tn)[NG], int cnt, double* __restrict__ C, int ldc,
-                                         const double* __restrict__ vadd = nullptr, int vcol = -1) {
+                                         const double* __restrict__ vadd = nullptr, int vcol = -1, const double* __restrict__ Cin = nullptr,
+                                         int ldcin = 0) {
   // (warp-uniform dispatch; NG bounds the tile count)
-  if (NG >= 4 && cnt == 4) mma_item_ng<TRANS_A, ACC, (NG >= 4 ? 4 : NG), KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol);
-  else if (NG >= 3 && cnt == 3) mma_item_ng<TRANS_A, ACC, (NG >= 3 ? 3 : NG), KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol);
-  else if (NG >= 2 && cnt == 2) mma_item_ng<TRANS_A, ACC, (NG >= 2 ? 2 : NG), KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol);
-  else if (cnt == 1) mma_item_ng<TRANS_A, ACC, 1, KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol);
+  if (NG >= 4 && cnt == 4)
+    mma_item_ng<TRANS_A, ACC, (NG >= 4 ? 4 : NG), KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol, Cin, ldcin);
+  else if (NG >= 3 && cnt == 3)
+    mma_item_ng<TRANS_A, ACC, (NG >= 3 ? 3 : NG), KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol, Cin, ldcin);
+  else if (NG >= 2 && cnt == 2)
+    mma_item_ng<TRANS_A, ACC, (NG >= 2 ? 2 : NG), KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol, Cin, ldcin);
+  else if (cnt == 1) mma_item_ng<TRANS_A, ACC, 1, KC, SYM_A, PERM_A, PERM_B>(lane, M, N, Krt, alpha, A, lda, tm, B, ldb, tn, C, ldc, vadd, vcol, Cin, ldcin);
 }
 
 // Work items of a symmetric 58 x 59 update (the [P | p] shape): row strip m needs the column tiles 0..m of the lower triangle plus tile 7,
@@ -194,92 +233,96 @@ struct SymItem {
 __constant__ SymItem kSymItems[13] = {
     {7, 4, {0, 1, 2, 3}}, {7, 4, {4, 5, 6, 7}}, {6, 4, {0, 1, 2, 3}}, {6, 4, {4, 5, 6, 7}}, {5, 4, {0, 1, 2, 3}}, {4, 4, {0, 1, 2, 3}}, {3, 4, {0, 1, 2, 3}},
     {2, 4, {0, 1, 2, 7}}, {5, 3, {4, 5, 7, 0}},   {1, 3, {0, 1, 7, 0}},   {4, 2, {4, 7, 0, 0}},   {0, 2, {0, 7, 0, 0}},   {3, 1, {7, 0, 0, 0}}};
-// P2 schedule (items per GEMM warp, -1 ends): warps 1-3 form R~ first (3 tiles each); warps 0 and 4 share their scheduler with the helper
-// warp, which runs the latency-bound factorisation during this phase, and get little work.
-__constant__ signed char kP2Sched[8][4] = {{7, 11, -1, -1}, {0, 13, -1, -1}, {1, 14, -1, -1}, {2, 15, -1, -1},
-                                           {18, -1, -1, -1}, {3, 16, 8, -1}, {4, 17, 9, -1},  {5, 6, 10, 12}};
-// the rest of W (item = 2 * row strip + {0: column tiles 0-3, 1: column tiles 4-6}) over the six worker warps
-__constant__ signed char kP1bItems[6][3] = {{0, 1, 15}, {2, 3, -1}, {4, 5, -1}, {6, 7, 8}, {9, 10, 11}, {12, 13, 14}};
-// P2 item order for the six worker warps (round robin): the fourteen 4-tile items first, the five short ones last
-__constant__ signed char kP2Order[19] = {0, 1, 2, 3, 4, 5, 6, 7, 13, 14, 15, 16, 17, 18, 8, 9, 10, 11, 12};
+// Item tables of a lane's four GEMM warps, by rank: rank 0 is the warp that shares its scheduler (and its fp64 / shuffle issue slots) with the
+// lane's helper warp, ranks 1-3 are the other three, which form R~ first (one 3-tile row strip each) and hand it to the helper.
+// P1b: the rest of W, column tiles 0..6 of the eight row strips (item = 2 * row strip + {0: column tiles 0-3, 1: column tiles 4-6}).
+__constant__ signed char kP1bItems[LANE_GEMM_WARPS][4] = {{0, 2, 4, 6}, {8, 1, 3, 5}, {10, 7, 9, 11}, {12, 14, 13, 15}};
+// P2: Q~ (the 13 symmetric items) and [S~ | r~] (items 13..18), 17 tiles for each R~ warp and 16 for rank 0; -1 ends
+__constant__ signed char kP2Sched[LANE_GEMM_WARPS][5] = {{0, 1, 2, 3, -1}, {4, 5, 6, 7, 12}, {13, 14, 15, 8, 10}, {16, 17, 18, 9, 11}};
 // stages without inputs (event nodes): only the 13 symmetric items
-__constant__ signed char kP2SchedNoInput[8][4] = {{0, 8, -1, -1}, {1, 9, -1, -1}, {2, 10, -1, -1}, {3, 11, -1, -1},
-                                                  {4, 12, -1, -1}, {5, -1, -1, -1}, {6, -1, -1, -1}, {7, -1, -1, -1}};
+__constant__ signed char kP2SchedNoInput[LANE_GEMM_WARPS][4] = {{0, 1, 12, -1}, {2, 3, 8, -1}, {4, 5, 9, -1}, {6, 7, 10, 11}};
 
 template <int NMAX>
-__device__ __forceinline__ void warp_chol_inverse_reg(int n, double* __restrict__ A, int lda, double reg, double* __restrict__ Linv, int ldl, int* ok);
+__device__ __forceinline__ void warp_chol_inverse_reg(int n, const double* A, int lda, double reg, double* Linv, int ldl, int* ok);
 
-__global__ void __launch_bounds__(BWD_THREADS, 1) riccati_bwd_kernel(QpDeviceView v) {
+// pairOff > 0: lane 1 of CTA c runs instance c + pairOff (the launch pairs instance c with c + ceil(B / 2)); pairOff = 0: lane 1 is idle.
+__global__ void __launch_bounds__(BWD_THREADS, 1) riccati_bwd_kernel(QpDeviceView v, int pairOff) {
   extern __shared__ double sm[];
-  const int inst = blockIdx.x;
-  if (v.skip && v.skip[inst * v.skipStride]) return;
-  const int N = v.N;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  double* PQ[2] = {sm, sm + PQ_D};
-  double* AB[2] = {sm + 2 * PQ_D, sm + 2 * PQ_D + AB_D};
-  double* W = AB[1] + AB_D;
-  double* Y[2] = {W + W_D, W + W_D + Y_D};
-  double* Rs[2] = {Y[1] + Y_D, Y[1] + Y_D + R_D};
-  double* Linv = Rs[1] + R_D;
-  unsigned long long* bar = reinterpret_cast<unsigned long long*>(Linv + R_D);   // [A | b | B], S of the next stage
-  unsigned long long* barQ = bar + 1;                                            // [Q | q] of the next stage
-  __shared__ int ok;
-  const bool gemmWarp = warp < GEMM_WARPS;
+  // warps 4 ln .. 4 ln + 3: the GEMM warps of lane ln; warp 8 + ln: its helper warp, on scheduler ln, which only one of its GEMM warps shares
+  const bool gemmWarp = warp < LANES * LANE_GEMM_WARPS;
+  const int ln = gemmWarp ? warp / LANE_GEMM_WARPS : warp - LANES * LANE_GEMM_WARPS;
+  const int lw = warp % LANE_GEMM_WARPS;                          // (GEMM warps) the warp's index in its lane = its scheduler
+  const int rank = lw == ln ? 0 : 1 + lw - (lw > ln);             // (GEMM warps) row of the item tables; ranks 1-3 form R~
+  const int lt = gemmWarp ? tid - 32 * LANE_GEMM_WARPS * ln : 32 * LANE_GEMM_WARPS + lane;   // thread index in the lane
+  if (ln == 1 && pairOff == 0) return;
+  const int inst = blockIdx.x + ln * pairOff;
+  if (inst >= v.B || (v.skip && v.skip[inst * v.skipStride])) return;
+  // every barrier below is the lane's own, so that a lane that returned above, or runs stages of another kind, never stalls the other one
+  const int barLane = 1 + 3 * ln, barRt = barLane + 1, barW = barLane + 2;
+  const auto laneSync = [&]() { named_sync(barLane, LANE_THREADS); };
+  const int N = v.N;
+  double* const P = sm + ln * LANE_D + PQ_OFF;
+  double* const AB = sm + ln * LANE_D + AB_OFF;
+  double* const W = sm + ln * LANE_D + W_OFF;
+  double* const Rt = sm + ln * LANE_D + RT_OFF;
+  double* const Rin = sm + ln * LANE_D + RIN_OFF;
+  const double* const Bk = AB + NXR * NX1R;
+  unsigned long long* bar = reinterpret_cast<unsigned long long*>(sm + LANES * LANE_D) + ln;   // [A | b | B] of the next stage
+  __shared__ int okLane[LANES];
+  int* const ok = &okLane[ln];
   const size_t iN = static_cast<size_t>(inst) * N, iN1 = static_cast<size_t>(inst) * (N + 1);
 
-  if (tid == 0) {
-    ok = 1;
+  if (lt == 0) {
+    *ok = 1;
     mbar_init(bar, 1);
-    mbar_init(barQ, 1);
     mbar_fence_init();
   }
-  int cur = 0;
   // terminal stage: [P_N | p_N] = [Q_N + reg I | q_N]
   {
     const double* QN = v.Q + (iN1 + N) * NXR * NXR;
-    for (int i = tid; i < NXR * NXR; i += blockDim.x) PQ[cur][i] = QN[i] + ((i % NXR == i / NXR) ? v.reg : 0.0);
-    for (int i = tid; i < NXR; i += blockDim.x) PQ[cur][NXR * NXR + i] = v.q[(iN1 + N) * NXR + i];
+    for (int i = lt; i < NXR * NXR; i += LANE_THREADS) P[i] = QN[i] + ((i % NXR == i / NXR) ? v.reg : 0.0);
+    for (int i = lt; i < NXR; i += LANE_THREADS) P[NXR * NXR + i] = v.q[(iN1 + N) * NXR + i];
   }
-  __syncthreads();
+  laneSync();
   // the cost-to-go of stage kk, symmetric from its lower triangle
-  auto storeP = [&](const double* Pc, int kk, int t0, int nt) {
+  auto storeP = [&](int kk, int t0, int nt) {
     for (int i = t0; i < NXR * NXR; i += nt) {
       const int r = i % NXR, c = i / NXR;
-      v.P[(iN1 + kk) * NXR * NXR + i] = r >= c ? Pc[r + c * NXR] : Pc[c + r * NXR];
+      v.P[(iN1 + kk) * NXR * NXR + i] = r >= c ? P[r + c * NXR] : P[c + r * NXR];
     }
-    for (int i = t0; i < NXR; i += nt) v.p[(iN1 + kk) * NXR + i] = Pc[NXR * NXR + i];
+    for (int i = t0; i < NXR; i += nt) v.p[(iN1 + kk) * NXR + i] = P[NXR * NXR + i];
   };
-  if (v.keepP) storeP(PQ[cur], N, tid, blockDim.x);
-  // Stage record k -> operand set `set`, issued by the helper warp only, in three parts: the bulk copies of [A | b | B] and S (one lane) as soon
-  // as that set is free; the bulk copies of [Q | q] once the buffer that takes them ([P | p] of the previous stage) is dead; the 8-byte cp.async
-  // of r and R (whose HBM addresses are only 8-byte aligned) after the factorisation.
-  auto prefetchBulk = [&](int k, int set) {
+  if (v.keepP) storeP(N, lt, LANE_THREADS);
+  // Stage record k, issued by the helper warp only, in three parts: the bulk copies of [A | b | B] (one lane) once the buffer is free, after
+  // the last read of the previous stage's; the L2 prefetch of the epilogue addends Q, q, S, r; the 8-byte cp.async of R (whose HBM address is
+  // only 8-byte aligned) after the factorisation, which is the last read of the previous R.
+  auto prefetchBulk = [&](int k) {
     const size_t sk = iN + k;
     const int nu = v.nu ? v.nu[sk] : NMR;
     if (lane == 0) {
       fence_proxy_async();
-      mbar_expect_tx(bar, static_cast<unsigned>((NXR * NX1R + NXR * nu + (nu > 0 ? NMR * NXR : 0)) * 8));
-      bulk_g2s(AB[set], v.A + sk * NXR * NXR, NXR * NXR * 8, bar);
-      bulk_g2s(AB[set] + NXR * NXR, v.b + sk * NXR, NXR * 8, bar);
-      if (nu > 0) {
-        bulk_g2s(AB[set] + NXR * NX1R, v.Bm + sk * NXR * NMR, static_cast<unsigned>(NXR * nu * 8), bar);
-        bulk_g2s(Y[set], v.S + sk * NMR * NXR, NMR * NXR * 8, bar);
-      }
+      mbar_expect_tx(bar, static_cast<unsigned>((NXR * NX1R + NXR * nu) * 8));
+      bulk_g2s(AB, v.A + sk * NXR * NXR, NXR * NXR * 8, bar);
+      bulk_g2s(AB + NXR * NXR, v.b + sk * NXR, NXR * 8, bar);
+      if (nu > 0) bulk_g2s(AB + NXR * NX1R, v.Bm + sk * NXR * NMR, static_cast<unsigned>(NXR * nu * 8), bar);
     }
   };
-  auto prefetchQ = [&](int k, double* qdst) {
+  auto prefetchAddends = [&](int k) {
+    const size_t sk = iN + k;
+    const int nu = v.nu ? v.nu[sk] : NMR;
     if (lane == 0) {
-      fence_proxy_async();
-      mbar_expect_tx(barQ, static_cast<unsigned>(NXR * NX1R * 8));
-      bulk_g2s(qdst, v.Q + (iN1 + k) * NXR * NXR, NXR * NXR * 8, barQ);
-      bulk_g2s(qdst + NXR * NXR, v.q + (iN1 + k) * NXR, NXR * 8, barQ);
+      bulk_prefetch_l2(v.Q + (iN1 + k) * NXR * NXR, NXR * NXR * 8);
+      bulk_prefetch_l2(v.q + (iN1 + k) * NXR, NXR * 8);
+      if (nu > 0) bulk_prefetch_l2(v.S + sk * NMR * NXR, NMR * NXR * 8);
+    } else if (lane < 3 && nu > 0) {
+      prefetch_l2(v.r + sk * NMR + (lane == 1 ? 0 : NMR - 1));   // r: 184 bytes, on at most two lines
     }
   };
-  auto prefetchSmall = [&](int k, int set) {
+  auto prefetchR = [&](int k) {
     const size_t sk = iN + k;
     const int nu = v.nu ? v.nu[sk] : NMR;
     if (nu > 0) {
-      if (lane < nu) __pipeline_memcpy_async(Y[set] + NMR * NXR + lane, v.r + sk * NMR + lane, 8);
       const double* Rg = v.R + sk * NMR * NMR;
       int c = 0, r = lane;   // (r, c) of element i = lane + 32 j, without divisions
       for (int i = lane; i < NMR * NMR; i += 32) {
@@ -287,157 +330,151 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) riccati_bwd_kernel(QpDeviceVie
           r -= NMR;
           ++c;
         }
-        __pipeline_memcpy_async(Rs[set] + r + c * LMR, Rg + i, 8);
+        __pipeline_memcpy_async(Rin + r + c * LMR, Rg + i, 8);
         r += 32;
       }
     }
     __pipeline_commit();
   };
-  unsigned parity = 0, parityQ = 0;
+  unsigned parity = 0;
   if (!gemmWarp) {
-    prefetchBulk(N - 1, 0);
-    prefetchQ(N - 1, PQ[1 - cur]);
-    prefetchSmall(N - 1, 0);
+    prefetchBulk(N - 1);
+    prefetchAddends(N - 1);
+    prefetchR(N - 1);
   }
   WB_CLOCK_BEGIN()
 
   for (int k = N - 1; k >= 0; --k) {
-    const int set = (N - 1 - k) & 1;
     const size_t sk = iN + k;
     const int nu = v.nu ? v.nu[sk] : NMR;
-    double* Pc = PQ[cur];
-    double* Pn = PQ[1 - cur];
-    double* ABk = AB[set];
-    double* Yk = Y[set];
-    double* Rk = Rs[set];
-    const double* Bk = ABk + NXR * NX1R;
     const int tilesN = (NX1R + nu + 7) >> 3;
-    // ---- [A | b | B], S, r, R of this stage have landed ----------------------------------------------------------------------------------------
+    // ---- [A | b | B] and R of this stage have landed ------------------------------------------------------------------------------------------
     if (!gemmWarp) __pipeline_wait_prior(0);
     mbar_wait(bar, parity);
     parity ^= 1;
-    __syncthreads();
+    laneSync();
     WB_TICK(1, 0)
     WB_TICK(20, 256)
     // ---- P1a: the columns of W = P [A | b | B] that R~ needs first: column tiles 7.. = [A_56 A_57 | b | B] (column b additionally gets p) --------
     if (gemmWarp) {
       const int tn[4] = {7, 8, 9, 10};
-      mma_item<false, false, 4, NXR, true, false, true>(lane, NXR, NX1R + nu, 0, 1.0, Pc, NXR, warp, ABk, NXR, tn, tilesN - 7, W, LWR, Pc + NXR * NXR, NXR);
+      for (int strip = lw; strip < 8; strip += LANE_GEMM_WARPS)
+        mma_item<false, false, 4, NXR, true, false, true>(lane, NXR, NX1R + nu, 0, 1.0, P, NXR, strip, AB, NXR, tn, tilesN - 7, W, LWR, P + NXR * NXR, NXR);
     } else if (v.keepP && k < N - 1) {
-      storeP(Pc, k + 1, lane, 32);   // (the cost-to-go of stage k+1 is complete and read-only until the [Q | q] copy below)
+      storeP(k + 1, lane, 32);   // (the cost-to-go of stage k+1 is complete and read-only until Q~ replaces it in P2)
     }
-    __syncthreads();
+    laneSync();
     WB_TICK(2, 0)
     WB_TICK(21, 256)
-    // ---- P1b / P2: helper warp: stream [A | b | B], S of stage k-1, then factorise R~ as soon as three GEMM warps hand it over -- the
-    //      factorisation (latency bound, one warp) runs WHILE the GEMM warps finish W (column tiles 0..6), and form Q~ (lower tiles) and [S~ | r~]
+    // ---- P1b / P2: helper warp: factorise R~ as soon as three GEMM warps hand it over -- the factorisation (latency bound, one warp) runs
+    //      WHILE the GEMM warps finish W (column tiles 0..6), and form Q~ (lower tiles) and [S~ | r~]
     if (!gemmWarp) {
-      if (k > 0) prefetchBulk(k - 1, 1 - set);
+      if (k > 0) prefetchAddends(k - 1);
       WB_TICK(22, 256)
       if (nu > 0) {
-        named_sync(1, 128);
+        named_sync(barRt, 128);
         WB_TICK(23, 256)
-        warp_chol_inverse_reg<24>(nu, Rk, LMR, v.reg, Linv, LMR, &ok);
+        warp_chol_inverse_reg<24>(nu, Rt, LMR, v.reg, Rt, LMR, ok);
         WB_TICK(24, 256)
       }
-      if (k > 0) prefetchSmall(k - 1, 1 - set);
+      if (k > 0) prefetchR(k - 1);
       WB_TICK(27, 256)
-    } else if ((warp & 3) != 0) {
-      // worker warps 1,2,3,5,6,7: the warps 0 and 4 share their scheduler (and its fp64 / shuffle issue slots) with the helper warp and sit this
-      // phase out while it factorises
-      const int wk = warp - 1 - (warp > 4);   // 0..5
-      if (nu > 0 && warp <= 3) {   // R~ = R + B'W_B
+    } else {
+      if (nu > 0 && rank > 0) {   // R~ = R + B'W_B
         const int tn[3] = {0, 1, 2};
-        mma_item<true, true, 3, NXR, false, true, false>(lane, nu, nu, 0, 1.0, Bk, NXR, warp - 1, W + LWR * NX1R, LWR, tn, 3, Rk, LMR);
+        mma_item<true, true, 3, NXR, false, true, false>(lane, nu, nu, 0, 1.0, Bk, NXR, rank - 1, W + LWR * NX1R, LWR, tn, 3, Rt, LMR, nullptr, -1, Rin,
+                                                         LMR);
         __threadfence_block();
-        named_arrive(1, 128);
+        named_arrive(barRt, 128);
       }
-      // the rest of W: column tiles 0..6 of the eight row strips, 16 items over the six workers (the three that formed R~ take two each)
-      for (int j = 0; j < 3; ++j) {
-        const int it = kP1bItems[wk][j];
-        if (it < 0) break;
+      for (int j = 0; j < 4; ++j) {
+        const int it = kP1bItems[rank][j];
         const int strip = it >> 1;
         if (it & 1) {
           const int tb[4] = {4, 5, 6, 0};
-          mma_item<false, false, 4, NXR, true, false, true>(lane, NXR, NX1R + nu, 0, 1.0, Pc, NXR, strip, ABk, NXR, tb, 3, W, LWR);
+          mma_item<false, false, 4, NXR, true, false, true>(lane, NXR, NX1R + nu, 0, 1.0, P, NXR, strip, AB, NXR, tb, 3, W, LWR);
         } else {
           const int ta[4] = {0, 1, 2, 3};
-          mma_item<false, false, 4, NXR, true, false, true>(lane, NXR, NX1R + nu, 0, 1.0, Pc, NXR, strip, ABk, NXR, ta, 4, W, LWR);
+          mma_item<false, false, 4, NXR, true, false, true>(lane, NXR, NX1R + nu, 0, 1.0, P, NXR, strip, AB, NXR, ta, 4, W, LWR);
         }
       }
-      named_sync(2, 32 * 6);   // W is complete (barrier of the six workers)
+      named_sync(barW, 32 * LANE_GEMM_WARPS);   // W is complete: P and W_B are dead
       WB_TICK(7, 32)
-      mbar_wait(barQ, parityQ);         // [Q | q] of this stage has landed in Pn
-      const int nItems = nu > 0 ? 19 : 13;
-      for (int it = wk; it < nItems; it += 6) {
-        const int id = nu > 0 ? kP2Order[it] : it;
-        if (id < 13) {
+      const double* Qg = v.Q + (iN1 + k) * NXR * NXR;
+      const double* qg = v.q + (iN1 + k) * NXR;
+      const double* Sg = v.S + sk * NMR * NXR;
+      const double* rg = v.r + sk * NMR;
+      const signed char* sched = nu > 0 ? kP2Sched[rank] : kP2SchedNoInput[rank];
+      const int nSched = nu > 0 ? 5 : 4;
+      for (int j = 0; j < nSched; ++j) {
+        const int id = sched[j];
+        if (id < 0) break;
+        if (id < 13) {   // Q~ = Q + A'W_A, q~ = q + A'v, over P
           const SymItem s = kSymItems[id];
           const int tn[4] = {s.n[0], s.n[1], s.n[2], s.n[3]};
-          mma_item<true, true, 4, NXR, false, true, false>(lane, NXR, NX1R, 0, 1.0, ABk, NXR, s.m, W, LWR, tn, s.cnt, Pn, NXR);
-        } else {
+          mma_item<true, true, 4, NXR, false, true, false>(lane, NXR, NX1R, 0, 1.0, AB, NXR, s.m, W, LWR, tn, s.cnt, P, NXR, qg, NXR, Qg, NXR);
+        } else {         // [S~ | r~] = [S | r] + B'[W_A | v], over W_B
           const int tm = (id - 13) >> 1, g = ((id - 13) & 1) * 4;
           const int tn[4] = {g, g + 1, g + 2, g + 3};
-          mma_item<true, true, 4, NXR, false, true, false>(lane, nu, NX1R, 0, 1.0, Bk, NXR, tm, W, LWR, tn, 4, Yk, NMR);
+          mma_item<true, true, 4, NXR, false, true, false>(lane, nu, NX1R, 0, 1.0, Bk, NXR, tm, W, LWR, tn, 4, W + Y_OFF, NMR, rg, NXR, Sg, NMR);
         }
       }
     }
-    parityQ ^= 1;
     WB_TICK(8, 0)
-    __syncthreads();
+    laneSync();
     WB_TICK(3, 0)
     WB_TICK(25, 256)
-    // [P | p] of the previous stage is dead now: its buffer takes [Q | q] of stage k-1 (needed at P2 of the next stage)
-    if (!gemmWarp && k > 0) prefetchQ(k - 1, Pc);
+    // [A | b | B] of this stage is dead now: its buffer takes stage k-1's, which lands behind P3 .. P5 (and behind the other lane)
+    if (!gemmWarp && k > 0) prefetchBulk(k - 1);
     double* Yl = W;
     double* Kout = W + KOUT_OFF;
     if (nu > 0) {
       // ---- P3: [Yl | yl] = L^-1 [S~ | r~] (into the W region) -----------------------------------------------------------------------------
       if (gemmWarp) {
-        for (int it = warp; it < 6; it += GEMM_WARPS) {
+        for (int it = lw; it < 6; it += LANE_GEMM_WARPS) {
           const int tm = it >> 1, g = (it & 1) * 4;
           const int tn[4] = {g, g + 1, g + 2, g + 3};
-          mma_item<false, false, 4, 0>(lane, nu, NX1R, nu, 1.0, Linv, LMR, tm, Yk, NMR, tn, 4, Yl, LMR);
+          mma_item<false, false, 4, 0>(lane, nu, NX1R, nu, 1.0, Rt, LMR, tm, W + Y_OFF, NMR, tn, 4, Yl, LMR);
         }
       }
-      __syncthreads();
+      laneSync();
       WB_TICK(4, 0)
       // ---- P4: [P | p] = [Q~ | q~] - Yl'[Yl | yl] (lower tiles) ; [K | k] = -L^-T [Yl | yl] -------------------------------------------------
       if (gemmWarp) {
-        for (int it = warp; it < 19; it += GEMM_WARPS) {
+        for (int it = lw; it < 19; it += LANE_GEMM_WARPS) {
           if (it < 8 || it >= 14) {
             const SymItem s = kSymItems[it < 8 ? it : it - 6];
             const int tn[4] = {s.n[0], s.n[1], s.n[2], s.n[3]};
-            mma_item<true, true, 4, 0>(lane, NXR, NX1R, nu, -1.0, Yl, LMR, s.m, Yl, LMR, tn, s.cnt, Pn, NXR);
+            mma_item<true, true, 4, 0>(lane, NXR, NX1R, nu, -1.0, Yl, LMR, s.m, Yl, LMR, tn, s.cnt, P, NXR);
           } else {
             const int j = it - 8, tm = j >> 1, g = (j & 1) * 4;
             const int tn[4] = {g, g + 1, g + 2, g + 3};
-            mma_item<true, false, 4, 0>(lane, nu, NX1R, nu, -1.0, Linv, LMR, tm, Yl, LMR, tn, 4, Kout, NMR);
+            mma_item<true, false, 4, 0>(lane, nu, NX1R, nu, -1.0, Rt, LMR, tm, Yl, LMR, tn, 4, Kout, NMR);
           }
         }
       }
-      __syncthreads();
+      laneSync();
       WB_TICK(5, 0)
     }
     // ---- P5: reg_prim on the diagonal, gains out -------------------------------------------------------------------------------------------
-    if (tid < NXR) Pn[tid + tid * NXR] += v.reg;
+    if (lt < NXR) P[lt + lt * NXR] += v.reg;
     if (nu > 0) {
-      for (int t = tid; t < NMR * NXR; t += blockDim.x) v.K[sk * NMR * NXR + t] = (t % NMR < nu) ? Kout[t] : 0.0;
-      for (int t = tid; t < nu; t += blockDim.x) v.kff[sk * NMR + t] = Kout[NMR * NXR + t];
+      for (int t = lt; t < NMR * NXR; t += LANE_THREADS) v.K[sk * NMR * NXR + t] = (t % NMR < nu) ? Kout[t] : 0.0;
+      for (int t = lt; t < nu; t += LANE_THREADS) v.kff[sk * NMR + t] = Kout[NMR * NXR + t];
     }
-    cur = 1 - cur;
     WB_TICK(6, 0)
     WB_TICK(26, 256)
     // (the barrier at the top of the next stage orders this phase before the next GEMM)
   }
-  __syncthreads();
-  if (v.keepP) storeP(PQ[cur], 0, tid, blockDim.x);
-  if (tid == 0) v.status[inst] = !ok;
+  laneSync();
+  if (v.keepP) storeP(0, lt, LANE_THREADS);
+  if (lt == 0) v.status[inst] = !*ok;
 }
 
-// warp_chol_inverse (dense.cuh) with reg added to the diagonal while loading
+// warp_chol_inverse (dense.cuh) with reg added to the diagonal while loading.  Linv may be A: each lane consumes all its loads of A in the
+// shuffles of column 0, which no lane completes before every lane has reached them, and the stores come after the last column.
 template <int NMAX>
-__device__ __forceinline__ void warp_chol_inverse_reg(int n, double* __restrict__ A, int lda, double reg, double* __restrict__ Linv, int ldl, int* ok) {
+__device__ __forceinline__ void warp_chol_inverse_reg(int n, const double* A, int lda, double reg, double* Linv, int ldl, int* ok) {
   const int lane = threadIdx.x & 31;
   double a[NMAX], z[NMAX];
 #pragma unroll
