@@ -244,6 +244,16 @@ int b200sqp_set_gait_schedule(b200sqp_handle h, int stateful, double phase_trans
  * GaitScheduleUpdater and trajectorySpread are the same functions on both families.  Whole-body handles: B200SQP_EINVAL. */
 int b200sqp_cen_set_gait_schedule(b200sqp_handle h, int stateful, double phase_transition_stance_time);
 
+/* Joint-torque cost of the whole-body OCP: the reference's JointTorqueCostCppAd (getJointTorqueCost(taskFile) added to the cost collection).
+ * weights [nj], MPC joint order (task.info joint_torque_weights): every intermediate node -- not PreEvent nodes, not the terminal node -- gets the
+ * Gauss-Newton cost 1/2 |sqrt(w) .* tau(x, u)|^2 with tau = computeJointTorques(x, u) (the map of b200sqp_joint_torques, evaluated with the
+ * instance's own MPC model: the handle's, or its B200SQP_PARAMS_MODEL record), scaled by the node's dt in the LQ approximation and in every
+ * line-search trial, like the other costs.  NULL or all-zero weights turn the term off (the default): the solve is then the same kernels and
+ * launches as without this call.  Takes effect at the next solve, for every instance, on the upload and the builder path alike; synchronous.
+ * Centroidal handles, a negative or non-finite weight: B200SQP_EINVAL, and nothing is applied.  B200SQP_ESTATE while a fleet is attached
+ * (set it before b200sqp_fleet_create). */
+int b200sqp_set_joint_torque_cost(b200sqp_handle h, const double* weights /* [nj] or NULL */);
+
 /* The window mode schedule [t0 - T, tf + T] the last b200sqp_build_instances used, in either mode: event_times [B][max_events],
  * mode_sequence [B][max_events + 1] (modes after the n_events[b] + 1 used entries are -1), n_events [B].  B200SQP_EINVAL when an instance has
  * more than max_events events. */

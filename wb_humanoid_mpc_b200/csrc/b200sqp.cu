@@ -25,6 +25,7 @@
 #include "wb_sim.cuh"
 #include "cen_dynamics.cuh"
 #include "wb_torque.cuh"
+#include "wb_torque_cost.cuh"
 #include "wb_mrt.cuh"
 #include "wb_devio.cuh"
 #include "cen_kernels.cuh"

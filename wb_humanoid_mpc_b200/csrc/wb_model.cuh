@@ -145,4 +145,35 @@ HD DV3 dmtv(const double* R, const double* dR, DV3 v) {
   return DV3{r[0] * v.x + r[3] * v.y + r[6] * v.z, r[1] * v.x + r[4] * v.y + r[7] * v.z, r[2] * v.x + r[5] * v.y + r[8] * v.z};
 }
 
+HD D1 dsin(D1 a) { return D1{sin(a.v), cos(a.v) * a.d}; }
+HD D1 dcos(D1 a) { return D1{cos(a.v), -sin(a.v) * a.d}; }
+HD D1 operator*(D1 a, double s) { return D1{a.v * s, a.d * s}; }
+HD D1 ddot(DV3 a, DV3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+HD DV3 operator*(D1 s, DV3 a) { return DV3{s * a.x, s * a.y, s * a.z}; }
+HD DV3 operator*(double s, DV3 a) { return DV3{s * a.x, s * a.y, s * a.z}; }
+HD DV3 dconst(double x, double y, double z) { return DV3{dmk(x), dmk(y), dmk(z)}; }
+struct DM3 {  // row-major
+  D1 m[9];
+};
+HD DV3 operator*(const DM3& A, DV3 v) {
+  return DV3{A.m[0] * v.x + A.m[1] * v.y + A.m[2] * v.z, A.m[3] * v.x + A.m[4] * v.y + A.m[5] * v.z, A.m[6] * v.x + A.m[7] * v.y + A.m[8] * v.z};
+}
+HD DM3 operator*(const DM3& A, const DM3& B) {
+  DM3 C;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) C.m[3 * i + j] = A.m[3 * i] * B.m[j] + A.m[3 * i + 1] * B.m[3 + j] + A.m[3 * i + 2] * B.m[6 + j];
+  return C;
+}
+HD DM3 dinv3(const DM3& A) {
+  const D1 c00 = A.m[4] * A.m[8] - A.m[5] * A.m[7], c01 = A.m[5] * A.m[6] - A.m[3] * A.m[8], c02 = A.m[3] * A.m[7] - A.m[4] * A.m[6];
+  const D1 id = dmk(1.0) / (A.m[0] * c00 + A.m[1] * c01 + A.m[2] * c02);
+  DM3 R;
+  R.m[0] = c00 * id; R.m[1] = (A.m[2] * A.m[7] - A.m[1] * A.m[8]) * id; R.m[2] = (A.m[1] * A.m[5] - A.m[2] * A.m[4]) * id;
+  R.m[3] = c01 * id; R.m[4] = (A.m[0] * A.m[8] - A.m[2] * A.m[6]) * id; R.m[5] = (A.m[2] * A.m[3] - A.m[0] * A.m[5]) * id;
+  R.m[6] = c02 * id; R.m[7] = (A.m[1] * A.m[6] - A.m[0] * A.m[7]) * id; R.m[8] = (A.m[0] * A.m[4] - A.m[1] * A.m[3]) * id;
+  return R;
+}
+
 }  // namespace b200sqp

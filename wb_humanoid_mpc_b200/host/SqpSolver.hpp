@@ -172,6 +172,16 @@ class SqpSolver {
   // see solveGroup: serialise the device phase of this object with every other SqpSolver of the process that also opted in
   void setExclusiveSolve(bool on) { exclusiveSolve_ = on; }
 
+  // problemPtr_->costPtr->add("jointTorqueCost", getJointTorqueCost(taskFile)) (WBMpcInterface.cpp): the joint-torque cost on every intermediate
+  // node of every instance, weights [nj] in MPC joint order (loadJointTorqueWeights); empty or all zeros: off.  Whole-body models only.
+  void setJointTorqueCost(const std::vector<double>& weights) {
+    if (!weights.empty() && static_cast<int>(weights.size()) != model_.nj)
+      throw std::invalid_argument("[SqpSolver] setJointTorqueCost: " + std::to_string(weights.size()) + " weights for " + std::to_string(model_.nj) + " joints");
+    for (auto& kv : groups_)
+      if (kv.second.h) check(b200sqp_set_joint_torque_cost(kv.second.h, weights.empty() ? nullptr : weights.data()));
+    jointTorqueWeights_ = weights;
+  }
+
   const PrimalSolution& primalSolution(int b) const { return primal_.at(b); }
   const std::vector<StepInfo>& getIterationsLog(int b) const {
     if (log_.at(b).empty()) throw std::runtime_error("[SqpSolver]: No performance log yet, no problem solved yet?");  // SqpSolver.cpp:174
@@ -278,6 +288,7 @@ class SqpSolver {
     if (!G.h)
       check(model_.centroidal ? b200sqp_cen_create(&model_.desc, &model_.cen, &settings_, device_, &G.h)
                               : b200sqp_create(&model_.desc, &settings_, device_, &G.h));
+    if (G.h && !jointTorqueWeights_.empty()) check(b200sqp_set_joint_torque_cost(G.h, jointTorqueWeights_.data()));
     const size_t B_ = static_cast<size_t>(Bg), n_ = static_cast<size_t>(n);
     if (G.capacity != Bg || G.nNodes != n) {
       // Invalidate first: if set_batch or a pinned allocation throws, the next call re-enters this branch
@@ -417,6 +428,7 @@ class SqpSolver {
   }
   static constexpr int kMaxGroups = 6;
   bool exclusiveSolve_ = false;
+  std::vector<double> jointTorqueWeights_;   // setJointTorqueCost (empty: off)
   std::mutex benchMutex_;
   HostModel model_;
   b200sqp_settings settings_;

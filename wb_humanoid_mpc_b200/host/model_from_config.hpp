@@ -301,6 +301,14 @@ struct Body {
 }  // namespace cfg
 
 // the MPC of WBMpcInterface (or, centroidal = true, of CentroidalMpcInterface) from its own files; gaitFile may be empty (no gait table)
+// WBMpcInterface::getJointTorqueCost: loadEigenMatrix(taskFile, "joint_torque_weights") into nj entries (MPC joint order); empty when the key is
+// absent.  Reading the key does not switch the term on (SqpSolver::setJointTorqueCost does), as the key alone does nothing in the reference.
+inline std::vector<double> loadJointTorqueWeights(const std::string& taskFile, int nj = 23) {
+  const cfg::Info task = cfg::parseInfo(taskFile);
+  if (!task.find("joint_torque_weights")) return {};
+  return task.column("joint_torque_weights", nj);
+}
+
 inline HostModel loadModelFromConfig(const std::string& urdfFile, const std::string& taskFile, const std::string& referenceFile,
                                      const std::string& gaitFile, bool centroidal = false) {
   using namespace cfg;

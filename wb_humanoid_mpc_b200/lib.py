@@ -138,6 +138,7 @@ EXPORTED_SYMBOLS = [
     "b200sqp_set_motion_manager",
     "b200sqp_download_motion_state",
     "b200sqp_cen_set_gait_schedule",
+    "b200sqp_set_joint_torque_cost",
     "b200sqp_cen_set_motion_manager",
     "b200sqp_default_rollout_settings",
     "b200sqp_rollout_policy",

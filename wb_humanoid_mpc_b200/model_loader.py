@@ -116,6 +116,16 @@ def info_matrix(tree: dict, name: str, rows: int, cols: int) -> np.ndarray:
     return out * scaling
 
 
+def joint_torque_weights(task_path, nj: int = 23) -> np.ndarray | None:
+    """joint_torque_weights of a task.info (WBMpcInterface::getJointTorqueCost: loadEigenMatrix into nj entries, MPC joint order; nj = the MPC
+    model's joint count, model["nj"]), or None when the key is absent.  Reading the key does not switch the term on: in the reference the cost
+    exists only where the interface adds it to the cost collection (B200SqpSolver.set_joint_torque_cost does that here)."""
+    task = parse_info(task_path)
+    if "joint_torque_weights" not in task:
+        return None
+    return info_matrix(task, "joint_torque_weights", nj, 1)[:, 0]
+
+
 def info_list(tree: dict, dotted: str) -> list[str]:
     blk = info_get(tree, dotted)
     items = []

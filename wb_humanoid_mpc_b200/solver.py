@@ -352,6 +352,15 @@ class B200SqpSolver:
         cycle's schedule), and the warm start is spread over the new schedule.  Takes effect at the next cold build."""
         _l.check(_l.lib().b200sqp_set_gait_schedule(self._h, C.c_int(int(stateful)), C.c_double(phase_transition_stance_time)))
 
+    def set_joint_torque_cost(self, weights=None):
+        """b200sqp_set_joint_torque_cost: the reference's JointTorqueCostCppAd on every intermediate node, weights [nj] in MPC joint order
+        (model_loader.joint_torque_weights reads them from a task.info); None or all zeros turns the term off.  Whole-body models only; takes
+        effect at the next solve."""
+        w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float64)
+        if w is not None and w.shape != (self.model["nj"],):
+            raise ValueError(f"set_joint_torque_cost: {w.shape} weights for {self.model['nj']} joints")
+        _l.check(_l.lib().b200sqp_set_joint_torque_cost(self._h, None if w is None else w.ctypes.data_as(_l.dp)))
+
     def set_motion_manager(self, enable: bool = True, filter_origin: float = 0.0):
         """b200sqp_set_motion_manager: the reference's ProceduralMpcMotionManager per instance on the device (stateful gait schedule needed).
         The velocity scales come from model["reference"], the gait ids of its seven states from the builder's gait table.  The cmd of every
