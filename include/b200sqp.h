@@ -122,7 +122,17 @@ void b200sqp_default_settings(b200sqp_settings* s);
 
 typedef struct b200sqp_solver_t* b200sqp_handle;
 
-/* SqpSolver::SqpSolver(settings, ocp, initializer) */
+/* Longest back-tracking ladder a handle serves: alpha_decay 0.95 with alpha_min 1e-4 takes 180 trials. */
+#define B200SQP_MAX_LS_TRIALS 200
+
+/* Number of trials of SqpSolver::takeStep's back-tracking (SqpSolver.cpp:527-565) for these settings: alpha = 1 is always tried (a do-while
+ * loop), then alpha *= alpha_decay -- by repeated multiplication -- while alpha >= alpha_min.  B200SQP_EINVAL, with a message, for settings
+ * b200sqp_create and b200sqp_cen_create reject: sqp_iteration outside [1, 1000]; a non-finite delta_tol, cost_tol, alpha_decay, alpha_min,
+ * gamma_c, g_max, g_min or armijo_factor; alpha_decay outside (0, 1); alpha_min <= 0; more than B200SQP_MAX_LS_TRIALS trials; more than 32
+ * trials with global_step = 1 (the candidates of the global-step mode, b200sqp_global_stats).  Needs no device. */
+int b200sqp_line_search_trials(const b200sqp_settings* settings, int32_t* n_trials);
+
+/* SqpSolver::SqpSolver(settings, ocp, initializer); the settings as b200sqp_line_search_trials checks them */
 int b200sqp_create(const b200sqp_model_desc* model, const b200sqp_settings* settings, int device, b200sqp_handle* out);
 void b200sqp_destroy(b200sqp_handle h);
 
@@ -150,10 +160,10 @@ int b200sqp_reset(b200sqp_handle h);
 
 /* SqpSolver::runImpl for every instance, ASYNCHRONOUS on `stream` (NULL = the legacy default stream): every kernel of up to sqp_iteration SQP
  * iterations is enqueued and the call returns; nothing on the host waits for the device.  The filter line search needs no host decision: an
- * instance needs at most ceil(log(alpha_min) / log(alpha_decay)) + 1 trials, all of them are enqueued, and the thread blocks of an instance
- * whose search has ended return at their first instruction (likewise every kernel for a converged instance).  b200sqp_wait -- or any entry
- * point that reads results or re-uses the handle (download*, get_stage_times, reset, upload / build_instances, set_batch, destroy) -- waits for
- * the stream first.  One solve per handle in flight; several handles on several streams overlap on the device.  (The global-step mode takes a
+ * instance needs at most b200sqp_line_search_trials trials (14 with the default settings), all of them are enqueued, and the thread blocks of
+ * an instance whose search has ended return at their first instruction (likewise every kernel for a converged instance).  b200sqp_wait -- or
+ * any entry point that reads results or re-uses the handle (download*, get_stage_times, reset, upload / build_instances, set_batch, destroy) --
+ * waits for the stream first.  One solve per handle in flight; several handles on several streams overlap on the device.  (The global-step mode takes a
  * host decision per candidate step and returns when the solve has finished.) */
 int b200sqp_solve(b200sqp_handle h, void* stream);
 /* Blocks until the last b200sqp_solve of this handle has finished; reports CUDA errors of the asynchronous work. */
@@ -167,8 +177,8 @@ int b200sqp_own_stream(b200sqp_handle h, void** stream);
 
 /* Global-step mode (settings.global_step = 1; SURVEY.md section 8e, not a reference semantic -- the reference searches per instance,
  * SqpSolver.cpp:517-565): one line-search step size per SQP iteration for the whole, possibly multi-GPU, batch.  Per iteration b200sqp_solve
- * walks the fixed ladder alpha_j = alpha_decay^j >= alpha_min from the largest candidate: one roll-out of every active instance, the
- * reference's filter test (FilterLinesearch.cpp:34-57), and
+ * walks the fixed ladder of the back-tracking trials (b200sqp_line_search_trials; at most 32 in this mode) from the largest candidate: one
+ * roll-out of every active instance, the reference's filter test (FilterLinesearch.cpp:34-57), and
  *   stats[j] = { #instances that accept alpha_j, sum of their trial merits, max trial constraint violation, #active instances }
  * combined over all ranks by two NCCL all-reduces (4 doubles SUM + 1 double MAX, on `stream`) when a communicator has been set; it stops at
  * the first candidate every active instance of every rank accepts and applies it (a zero step when none is).  Every rank takes the same
@@ -386,9 +396,9 @@ typedef struct b200sqp_iter_log {
 
 /* primalSolution / getRiccatiFeedback / getIterationsLog:
  *   x [B][n_nodes][nx], u [B][n_nodes-1][nu], K [B][n_nodes-1][nu*nx] (remapped gains, may be NULL),
- *   log [B][sqp_iteration], n_iter [B], status [B]: 0 ok; 1 QP failed (Cholesky of the projected input Hessian, NaN); 2 a whole-body
- *   constraint Jacobian D lost full row rank under Eigen::FullPivLU's threshold (the reference's luConstraintProjection would continue with a
- *   larger null space; this path reports it).  Any non-zero status makes the call return B200SQP_EQP. Synchronises. */
+ *   log [B][sqp_iteration] (rows from n_iter on are zeros), n_iter [B], status [B]: 0 ok; 1 QP failed (Cholesky of the projected input
+ *   Hessian, NaN); 2 a whole-body constraint Jacobian D lost full row rank under Eigen::FullPivLU's threshold (the reference's
+ *   luConstraintProjection would continue with a larger null space; this path reports it).  Any non-zero status makes the call return B200SQP_EQP. Synchronises. */
 int b200sqp_download(b200sqp_handle h, double* x, double* u, double* K, b200sqp_iter_log* log, int32_t* n_iter, int32_t* status);
 
 /* SqpSolver::getValueFunction data (needs settings.create_value_function): quadratic cost-to-go of the last iteration's QP,

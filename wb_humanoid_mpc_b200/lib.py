@@ -147,6 +147,7 @@ EXPORTED_SYMBOLS = [
     "b200sqp_set_comm",
     "b200sqp_global_stats",
     "b200sqp_global_ladder",
+    "b200sqp_line_search_trials",
     "b200sqp_download",
     "b200sqp_download_value_function",
     "b200sqp_centroidal_flow_map",
