@@ -64,7 +64,7 @@ def test_lq_node_blocks_and_projection(model, wb, contact):
         assert rel(e[k], pr[k]) < 1e-10, k
 
 
-@pytest.mark.parametrize("contact", [(1, 1), (1, 0), (0, 0)])
+@pytest.mark.parametrize("contact", [(1, 1), (1, 0), (0, 1), (0, 0)])
 @pytest.mark.parametrize("mode", [1, 2])
 def test_cuda_k1b_schedules_equal_the_one_pass_schedule(model, wb, contact, mode):
     """The GPU runs K1b as lu_kernel + wb_node_b1.inc (projection, dynamics) + wb_node_b2.inc (cost; mode 2: Q accumulated in place in its
