@@ -82,6 +82,14 @@ def cen_node(desc, cdesc, x, u, xnext, xref, dt, contact, swing, impact, arm_pha
                 Pu=Pu.T[:, :n].copy(), Px=Px.T.copy(), u0=u0, nut=n, perf=perf, raw=unpack_raw_blocks(raw, CX, NU))
 
 
+def cen_flow(desc, cdesc, x, u):
+    """cen_flow_kernel's value lane (cenFlowDual) on the host: xdot of one centroidal (x, u)"""
+    xd = np.zeros(35)
+    rc = lib().emu_cen_flow(C.byref(desc), C.byref(cdesc), _p(F(x)), _p(F(u)), _p(xd))
+    assert rc == 0
+    return xd
+
+
 def joint_torques(desc, x, u):
     tau, qddb = np.zeros(23), np.zeros(6)
     rc = lib().emu_joint_torques(C.byref(desc), _p(F(x)), _p(F(u)), _p(tau), _p(qddb))

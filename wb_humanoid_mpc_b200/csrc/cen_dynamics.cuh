@@ -8,9 +8,9 @@
 // differentiated by CppAD in the reference.  Layout: x = [h/m (lin 3, ang 3); base position 3; Euler ZYX 3; joints nj],
 // u = [wrench_l (f, tau); wrench_r; qdot_j].
 //
-// Own formulation (not a port of Pinocchio): everything in WORLD coordinates, so that column k of the centroidal momentum matrix is a
-// closed form of the composite of the subtree moved by coordinate k -- mass M, first moment mu = sum m c, second moment about the world
-// origin J = sum (Ic + m (|c|^2 1 - c c')) -- for a unit rotation w about an axis through p:
+// Own formulation (not a port of Pinocchio): world axes, positions measured from the base position (the map is invariant to it), so that
+// column k of the centroidal momentum matrix is a closed form of the composite of the subtree moved by coordinate k -- mass M, first moment
+// mu = sum m c, second moment about the base position J = sum (Ic + m (|c|^2 1 - c c')) -- for a unit rotation w about an axis through p:
 //   h_lin = w x (mu - M p),   L_O = J w - mu x (w x p),   L_G = L_O - G x h_lin      (translations: h_lin = m e_k, L_G = 0)
 // One warp per instance: lane 0 evaluates the value and the analytic columns (the map is affine in hbar, the wrenches and qdot_j and
 // invariant to the base position), lanes 1..26 each carry one tangent (3 Euler angles + 23 joints) through the same code as a
@@ -57,7 +57,9 @@ HD void cenFlowDual(const CenModel& m, const double* x, const double* u, int dir
     R[0].m[0] = c0 * c1; R[0].m[1] = c0 * s1 * s2 - s0 * c2; R[0].m[2] = c0 * s1 * c2 + s0 * s2;
     R[0].m[3] = s0 * c1; R[0].m[4] = s0 * s1 * s2 + c0 * c2; R[0].m[5] = s0 * s1 * c2 - c0 * s2;
     R[0].m[6] = -s1;     R[0].m[7] = c1 * s2;                R[0].m[8] = c1 * c2;
-    p[0] = DV3{q[0], q[1], q[2]};
+    // positions are measured from the base position: the map is invariant to it, and second moments J about a distant world origin would
+    // cancel digits in L_G (a base 1 km out lost 7 of them)
+    p[0] = dconst(0, 0, 0);
     ax[0] = dconst(0, 0, 0);
   }
 #pragma unroll 1

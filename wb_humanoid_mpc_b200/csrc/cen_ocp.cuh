@@ -64,12 +64,15 @@ struct CenKin {
 };
 
 HD void cenKinematics(const CenModel& m, const D1* q, CenKin& k) {
+  // placements are formed relative to the base position and moved to the world at the end: the subtree second moments J are taken about the
+  // base, so that a base far from the world origin (|c|^2 of 1e6 m^2 at 1 km) does not cancel digits in the centroidal momentum matrix
+  const DV3 base{q[0], q[1], q[2]};
   {
     const D1 c0 = dcos(q[3]), s0 = dsin(q[3]), c1 = dcos(q[4]), s1 = dsin(q[4]), c2 = dcos(q[5]), s2 = dsin(q[5]);
     k.R[0].m[0] = c0 * c1; k.R[0].m[1] = c0 * s1 * s2 - s0 * c2; k.R[0].m[2] = c0 * s1 * c2 + s0 * s2;
     k.R[0].m[3] = s0 * c1; k.R[0].m[4] = s0 * s1 * s2 + c0 * c2; k.R[0].m[5] = s0 * s1 * c2 - c0 * s2;
     k.R[0].m[6] = -s1;     k.R[0].m[7] = c1 * s2;                k.R[0].m[8] = c1 * c2;
-    k.p[0] = DV3{q[0], q[1], q[2]};
+    k.p[0] = dconst(0, 0, 0);
     k.ax[0] = dconst(0, 0, 0);
     const DV3 Scol[3] = {DV3{-s1, c1 * s2, c1 * c2}, DV3{dmk(0.0), c2, -s2}, DV3{dmk(1.0), dmk(0.0), dmk(0.0)}};
     for (int e = 0; e < 3; ++e) k.Sw[e] = k.R[0] * Scol[e];
@@ -90,6 +93,8 @@ HD void cenKinematics(const CenModel& m, const D1* q, CenKin& k) {
     k.ax[i] = k.R[i] * dconst(a[0], a[1], a[2]);
   }
   if (m.modelType == 1) {
+#pragma unroll 1
+    for (int i = 0; i < NB; ++i) k.p[i] = k.p[i] + base;
     // updateCentroidalDynamics, SingleRigidBodyDynamics branch (ocs2_centroidal_model/src/ModelHelperFunctions.cpp:61-79): Ag = [Ab 0] from the
     // nominal centroidal inertia and com offset carried with the base; the frame placements above still follow the full kinematics
     const DV3 rw = k.R[0] * dconst(m.comToBaseNominal[0], m.comToBaseNominal[1], m.comToBaseNominal[2]);
@@ -147,8 +152,7 @@ HD void cenKinematics(const CenModel& m, const D1* q, CenKin& k) {
     for (int e = 0; e < 6; ++e) k.J[pa][e] = k.J[pa][e] + k.J[i][e];
   }
   k.mass = k.M[0];
-  k.G = (dmk(1.0) / k.mass) * k.mu[0];
-  k.Gcom = k.G;
+  const DV3 Grel = (dmk(1.0) / k.mass) * k.mu[0];
 #pragma unroll 1
   for (int c = 3; c < NV; ++c) {
     const int b = (c < 6) ? 0 : c - 5;
@@ -156,10 +160,15 @@ HD void cenKinematics(const CenModel& m, const D1* q, CenKin& k) {
     const DV3 hl = dcross(w, k.mu[b] - k.M[b] * k.p[b]);
     const D1* Jb = k.J[b];
     const DV3 Jw{Jb[0] * w.x + Jb[1] * w.y + Jb[2] * w.z, Jb[1] * w.x + Jb[3] * w.y + Jb[4] * w.z, Jb[2] * w.x + Jb[4] * w.y + Jb[5] * w.z};
-    const DV3 LG = Jw - dcross(k.mu[b], dcross(w, k.p[b])) - dcross(k.G, hl);
+    const DV3 LG = Jw - dcross(k.mu[b], dcross(w, k.p[b])) - dcross(Grel, hl);
     k.Ag[0][c - 3] = hl.x; k.Ag[1][c - 3] = hl.y; k.Ag[2][c - 3] = hl.z;
     k.Ag[3][c - 3] = LG.x; k.Ag[4][c - 3] = LG.y; k.Ag[5][c - 3] = LG.z;
   }
+  // world placements and centre of mass (mu and J stay about the base: nothing after this reads them)
+#pragma unroll 1
+  for (int i = 0; i < NB; ++i) k.p[i] = k.p[i] + base;
+  k.G = Grel + base;
+  k.Gcom = k.G;
 }
 
 // flow map on duals given the kinematics of q = x[6..35)
