@@ -629,6 +629,42 @@ int b200sqp_download_dev(b200sqp_handle h, double* x, double* u, double* K, int3
 int b200sqp_fleet_download_dev(b200sqp_fleet f, int max_nodes, double* x, double* u, double* K, int32_t* status, int32_t* n_nodes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * MRT-side queries of the last solve: MPC_MRT_Interface::getValueFunction(time, state) (= SqpSolver::getValueFunction, SqpSolver.cpp:172-191)
+ * and getLinearFeedbackGain(time) (LinearController::getFeedbackGain), batched, at one time t shared by every instance.  Per instance b, on its
+ * own plan (its own node count on a fleet):
+ *   (idx, alpha) = LinearInterpolation::timeSegment(t_nodes[b], t): t before the first node holds the first node, t past the last node the
+ *   last, and a segment not longer than 2 weakEpsilon (a PreEvent / PostEvent pair) snaps to its nearer end;
+ *   vf_dfdxx [B][nx*nx] = alpha P[idx] + (1 - alpha) P[idx + 1] entry-wise (column-major), P as b200sqp_download_value_function returns it;
+ *   vf_dfdx [B][nx]     = alpha p[idx] + (1 - alpha) p[idx + 1], then dfdx_r += dfdxx_rc x_c for c = 0 .. nx-1 in that order (the re-centring
+ *                         at x); the constant f is not produced (the reference sets it to 0);
+ *   K [B][nu*nx]        = alpha K_src(idx) + (1 - alpha) K_src(idx + 1) entry-wise (column-major), src the stage whose gain node k carries
+ *                         (toPrimalSolution: PreEvent nodes and the terminal node take the stage before them) -- the gain the linear policy of
+ *                         b200sqp_rollout_policy / b200sqp_joint_actions uses at t.
+ *   Every product and sum is rounded on its own, in the order above, so the results equal that formula on the host bit for bit.
+ *   x [B][nx]: the state dfdx is re-centred at, read only when vf_dfdx is wanted; NULL: the end state of the last roll-out (as
+ *   b200sqp_joint_actions(robot_state = NULL)).  Centroidal handles: nx = nu = 35 (the leading 35 rows and columns of the device blocks).
+ *   Outputs: each may be NULL; with all three NULL the call returns 0 and enqueues nothing.  Caller order on fleets.
+ * b200sqp_mrt_query / b200sqp_fleet_mrt_query: host arrays, ASYNCHRONOUS on `stream` like b200sqp_joint_actions (x is copied before the call
+ *   returns; the outputs are valid after b200sqp_wait / b200sqp_fleet_wait).
+ * b200sqp_mrt_query_dev / b200sqp_fleet_mrt_query_dev: x and every output in device memory, under the rules of the device-pointer I/O section
+ *   (pointer check, stream waits, event after the call's work).
+ * The query reads the plan, the cost-to-go, the gains and the simulated state and writes none of them: a later build, roll-out, joint-action
+ * call or solve behaves as if it had not been made.
+ * B200SQP_EINVAL: null handle, non-finite t, a _dev pointer that is not device memory.  B200SQP_ESTATE: nothing solved yet (a fleet before its
+ * first build); vf_dfdxx or vf_dfdx with settings.create_value_function = 0; K with settings.use_feedback_policy = 0 (a feed-forward policy, where
+ * the reference throws); x = NULL with vf_dfdx and no roll-out of the batch.  The handle entry points return B200SQP_ESTATE while a fleet is
+ * attached.
+ * b200sqp_fleet_download_value_function: b200sqp_download_value_function of a fleet, in caller order with max_nodes node rows per instance
+ *   (the rows past n_nodes[b] zero): P [B][max_nodes][nx*nx], p [B][max_nodes][nx], n_nodes [B] (may be NULL).  Synchronises.
+ *   B200SQP_EINVAL for a null P or p or an instance with more than max_nodes nodes; B200SQP_ESTATE as b200sqp_download_value_function.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int b200sqp_mrt_query(b200sqp_handle h, double t, const double* x, double* vf_dfdxx, double* vf_dfdx, double* K, void* stream);
+int b200sqp_fleet_mrt_query(b200sqp_fleet f, double t, const double* x, double* vf_dfdxx, double* vf_dfdx, double* K, void* stream);
+int b200sqp_mrt_query_dev(b200sqp_handle h, double t, const double* x, double* vf_dfdxx, double* vf_dfdx, double* K, void* stream);
+int b200sqp_fleet_mrt_query_dev(b200sqp_fleet f, double t, const double* x, double* vf_dfdxx, double* vf_dfdx, double* K, void* stream);
+int b200sqp_fleet_download_value_function(b200sqp_fleet f, int max_nodes, double* P, double* p, int32_t* n_nodes);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Per-instance gains: the reference's GainsReceiver (humanoid_centroidal_mpc_ros2 src/gains/GainsReceiver.cpp), a synchronized module whose
  * preSolverRun writes the newest gains message into the OCP's cost and soft-constraint terms, per instance of the batch on the device.
  * A gain set belongs to one instance index of the built batch (caller order, also on a fleet) and takes effect at that instance's next solve,

@@ -28,6 +28,7 @@
 #include "wb_torque_cost.cuh"
 #include "wb_mrt.cuh"
 #include "wb_devio.cuh"
+#include "wb_query.cuh"
 #include "cen_kernels.cuh"
 #include "cen_host.cuh"
 #include "wb_gains.cuh"

@@ -189,6 +189,11 @@ EXPORTED_SYMBOLS = [
     "b200sqp_fleet_joint_actions_dev",
     "b200sqp_download_dev",
     "b200sqp_fleet_download_dev",
+    "b200sqp_mrt_query",
+    "b200sqp_fleet_mrt_query",
+    "b200sqp_mrt_query_dev",
+    "b200sqp_fleet_mrt_query_dev",
+    "b200sqp_fleet_download_value_function",
     "b200sqp_default_gains",
     "b200sqp_set_gains",
     "b200sqp_download_gains",

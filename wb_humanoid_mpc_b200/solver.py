@@ -136,6 +136,42 @@ def _joint_actions_device(fn, h, device, B, nx, nu, nj, t, robot_state, use_poli
     return o
 
 
+def _mrt_query(fn, h, wait, B, nx, nu, t, x, value, gain, stream) -> dict:
+    """the host entry point of the MRT queries; dfdxx / K come back column-major and are returned as [B, nx, nx] / [B, nu, nx]"""
+    xs = None if x is None or not value else _f(x)
+    if xs is not None:
+        assert xs.shape == (B, nx), xs.shape
+    P = np.zeros((B, nx, nx)) if value else None
+    p = np.zeros((B, nx)) if value else None
+    K = np.zeros((B, nx, nu)) if gain else None
+    opt = lambda a: None if a is None else _p(a)
+    _l.check(fn(h, C.c_double(t), opt(xs), opt(P), opt(p), opt(K), C.c_void_p(stream or 0)))
+    wait()
+    out = {}
+    if value:
+        out["dfdxx"], out["dfdx"] = np.swapaxes(P, -1, -2).copy(), p
+    if gain:
+        out["K"] = np.swapaxes(K, -1, -2).copy()
+    return out
+
+
+def _mrt_query_device(fn, h, device, B, nx, nu, t, x, value, gain, stream) -> dict:
+    import torch
+
+    xs = None if x is None or not value else check_device_tensor(x, "x", device, torch.float64, (B, nx))
+    f64 = torch.float64
+    P = torch.empty((B, nx, nx), dtype=f64, device=device) if value else None
+    p = torch.empty((B, nx), dtype=f64, device=device) if value else None
+    K = torch.empty((B, nx, nu), dtype=f64, device=device) if gain else None
+    _l.check(fn(h, C.c_double(t), _vp(xs), _vp(P), _vp(p), _vp(K), _stream(device, stream)))
+    out = {}
+    if value:
+        out["dfdxx"], out["dfdx"] = P.transpose(-1, -2), p
+    if gain:
+        out["K"] = K.transpose(-1, -2)
+    return out
+
+
 def _set_gains(fn, h, indices, gains):
     idx = np.ascontiguousarray(np.atleast_1d(indices), dtype=np.int32)
     rec = None if gains is None else abi.pack_gains(gains, idx.size if np.ndim(gains["final_cost_active"]) == 0 else None)
@@ -560,6 +596,20 @@ class B200SqpSolver:
         return _joint_actions_device(_l.lib().b200sqp_joint_actions_dev, self._h, torch.device("cuda", self.device), self.batch, self.nx, self.nu,
                                      self.model["nj"], t, robot_state, use_policy, out, stream)
 
+    def mrt_query(self, t: float, x=None, value: bool = True, gain: bool = True, stream=None) -> dict:
+        """MPC_MRT_Interface::getValueFunction(t, x) and getLinearFeedbackGain(t) of the last solve for every instance (b200sqp_mrt_query):
+        value -> dfdxx [B, nx, nx], dfdx [B, nx] (the cost-to-go interpolated at t, re-centred at x [B, nx]; x = None: the end state of the
+        last roll-out), gain -> K [B, nu, nx].  Needs settings.create_value_function / use_feedback_policy for what is asked.  Waits."""
+        return _mrt_query(_l.lib().b200sqp_mrt_query, self._h, self.wait, self.batch, self.nx, self.nu, t, x, value, gain, stream)
+
+    def mrt_query_device(self, t: float, x=None, value: bool = True, gain: bool = True, stream=None) -> dict:
+        """mrt_query in device memory (b200sqp_mrt_query_dev): x a float64 CUDA tensor [B, nx] or None, enqueued on `stream` (default: the
+        current torch stream) without waiting; CUDA tensors dfdxx [B, nx, nx] and K [B, nu, nx] (transposed views) and dfdx [B, nx]"""
+        import torch
+
+        return _mrt_query_device(_l.lib().b200sqp_mrt_query_dev, self._h, torch.device("cuda", self.device), self.batch, self.nx, self.nu, t, x,
+                                 value, gain, stream)
+
     def primal_solution_device(self, with_gains: bool | None = None, stream=None) -> dict:
         """primal_solution in device memory (b200sqp_download_dev), enqueued on `stream` without waiting: CUDA tensors {x [B, n, nx],
         u [B, n-1, nu], status [B] (int32, the per-instance solve status; nothing is raised), K [B, n-1, nu, nx] (a transposed view) with gains}"""
@@ -867,6 +917,26 @@ class B200SqpFleet:
 
         return _joint_actions_device(_l.lib().b200sqp_fleet_joint_actions_dev, self._f, torch.device("cuda", self.solver.device), self.batch, self.nx,
                                      self.nu, self.model["nj"], t, robot_state, use_policy, out, stream)
+
+    def mrt_query(self, t: float, x=None, value: bool = True, gain: bool = True, stream=None) -> dict:
+        """B200SqpSolver.mrt_query (b200sqp_fleet_mrt_query), caller order, each instance on its own plan"""
+        return _mrt_query(_l.lib().b200sqp_fleet_mrt_query, self._f, self.wait, self.batch, self.nx, self.nu, t, x, value, gain, stream)
+
+    def mrt_query_device(self, t: float, x=None, value: bool = True, gain: bool = True, stream=None) -> dict:
+        """B200SqpSolver.mrt_query_device (b200sqp_fleet_mrt_query_dev), caller order"""
+        import torch
+
+        return _mrt_query_device(_l.lib().b200sqp_fleet_mrt_query_dev, self._f, torch.device("cuda", self.solver.device), self.batch, self.nx,
+                                 self.nu, t, x, value, gain, stream)
+
+    def value_function(self, max_nodes: int | None = None):
+        """B200SqpSolver.value_function of the fleet (b200sqp_fleet_download_value_function): (P [B, m, nx, nx], p [B, m, nx], n_nodes [B]) with
+        m = max_nodes or max(n_nodes), rows past an instance's n_nodes zero"""
+        B, nx = self.batch, self.nx
+        m = int(self.n_nodes.max()) if max_nodes is None else int(max_nodes)
+        P, p, n = np.zeros((B, m, nx, nx)), np.zeros((B, m, nx)), np.zeros(B, dtype=np.int32)
+        _l.check(_l.lib().b200sqp_fleet_download_value_function(self._f, C.c_int(m), _p(P), _p(p), n.ctypes.data_as(_l.ip)))
+        return np.swapaxes(P, -1, -2).copy(), p, n
 
     def primal_solution_device(self, with_gains: bool | None = None, stream=None) -> dict:
         """B200SqpSolver.primal_solution_device (b200sqp_fleet_download_dev): x [B, m, nx], u [B, m - 1, nu] (m = max(n_nodes), rows past an
